@@ -1,6 +1,11 @@
-"""bench.py — headline benchmark of the B200 hot paths (contract: see the task statement / DESIGN.md §5).
+"""bench.py — headline benchmark of the hot paths on the H100 (DESIGN.md §5).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
+
+--dump-outputs DIR: after the timed steps, write what the timed neighbor_sample call returned in its last step (row,
+col, node_id, edge_id as float64 — exact for ids < 2^53 — and the per-hop counts) and a fixed, seeded sample of rows of
+the last segment_matmul result (float32) as DIR/<name>.npy.  Inputs are generated from fixed seeds, so two builds run
+with the same arguments can be compared output for output.
 
 metric  : sampled edges/s of pyg_lib.sampler.neighbor_sample.
 N = 1   : BASELINE.json configs[1] — ogbn-products-shaped CSR (2,449,029 nodes / 123,718,280 edges, int64), fan-out
@@ -8,8 +13,9 @@ N = 1   : BASELINE.json configs[1] — ogbn-products-shaped CSR (2,449,029 nodes
           `value` = graph AND seeds resident in HBM (each call still ends with the API's own host sync, because the op
           returns Python lists); `e2e` = the same through the public API with HOST buffers: pinned seeds -> device
           every step, sampled (row, col, node_id, edge_id) -> pinned host memory every step.
-          Same JSON line: `parity` (gates run BEFORE timing, against the reference's CPU implementation in a
-          subprocess: C2 bit-exact incl. generator state, C3 bf16 <= 1e-3 rel. Frobenius and <= 1 ulp), `roofline`
+          Same JSON line: `parity` (gates run BEFORE timing, against answers the reference's CPU implementation gave
+          on these inputs, tests/golden/config_parity.json: C2 bit-exact incl. generator state, C3 bf16 <= 1e-3 rel.
+          Frobenius and <= 1 ulp on a fixed sample of rows), `roofline`
           (dominant sampler kernel, device-timed, actual edges), `cpu_baseline`, `segment_matmul` (configs[2]: 64
           relations, N = 2^20 ragged rows, 128 -> 128 bf16: TFLOP/s, roofline, its own e2e), `c5_single_gpu`
           (configs[4]'s graph and batch on one GPU: the strong-scaling baseline of the N > 1 lines).
@@ -161,41 +167,40 @@ def reference_arm(a):
 
 
 # ------------------------------------------------------------------------------------------------ parity gates
-def parity_gates(P, dev, rowptr_c, col_c, rowptr, col, perm, with_matmul=True):
-    """BASELINE.md 4.4: parity before timing, at config size, against the reference in a subprocess."""
+def parity_gates(P, dev, rowptr, col, perm, with_matmul=True):
+    """BASELINE.md 4.4: parity before timing, at config size, against what the reference answered on these inputs
+    (tests/golden/make_golden_config.py)."""
     import torch
     from graphs import ragged_ptr
-    from refproc import RefSession, accumulation_bound, compare_homo, lowp_ulp_excess, rng_prefix
+    from refproc import accumulation_bound, compare_homo_golden, digest, golden, golden_rows, lowp_ulp_excess, rng_prefix
     res = {}
     seeds = [perm[b * BATCH:(b + 1) * BATCH].clone() for b in (0, 1)]
-    with RefSession() as rs:
-        ref = rs.run(dict(kind='homo', rowptr=rs.share(rowptr_c), col=rs.share(col_c), seeds=seeds, num_neighbors=FANOUT, rng_seed=777))
-        saved = torch.get_rng_state()
-        torch.manual_seed(777)
-        cmp = [compare_homo(P.sampler.neighbor_sample(rowptr, col, s.to(dev), FANOUT), c) for s, c in zip(seeds, ref['calls'])]
-        rng_ok = bool(torch.equal(rng_prefix(), ref['rng_after']))
-        torch.set_rng_state(saved)
-        res['c2_neighbor_sample'] = {'against': ref['kind'], 'calls': len(cmp), 'edges': sum(c['edges'] for c in cmp),
-                                     'bit_exact': all(c['bit_exact'] for c in cmp), 'generator_state_equal': rng_ok,
-                                     'mismatch': sum((c['mismatch'] for c in cmp), [])}
-        ok = res['c2_neighbor_sample']['bit_exact'] and rng_ok
-        if with_matmul:
-            Nn, K, M, B = 1 << 20, 128, 128, 64
-            g = torch.Generator().manual_seed(0)
-            x = torch.randn(Nn, K, generator=g).to(torch.bfloat16)
-            w = (torch.randn(B, K, M, generator=g) / K ** 0.5).to(torch.bfloat16)
-            ptr = ragged_ptr(Nn, B, 100)
-            y_path = rs.out_file(Nn * M, torch.bfloat16)
-            refm = rs.run(dict(kind='matmul', x=rs.share(x), w=rs.share(w), ptr=ptr, y_path=y_path))
-            y_ref = torch.from_file(y_path, shared=False, size=Nn * M, dtype=torch.bfloat16).view(Nn, M)
-            y = P.ops.segment_matmul(x.to(dev), ptr.to(dev), w.to(dev)).cpu()
-            rel = float((y.float() - y_ref.float()).norm() / y_ref.float().norm())
-            ulp = lowp_ulp_excess(y, y_ref, accumulation_bound(x.to(dev), ptr, w.to(dev)).cpu())
-            res['c3_segment_matmul'] = {'against': refm['kind'], 'rel_frobenius': rel, 'max_ulp': ulp,
-                                        'tolerance': '<= 1e-3 and <= 1 bf16 ulp (+ the fp32 summation-order bound 2K 2^-24 |x||w| for cancelling results)',
-                                        'pass': rel <= 1e-3 and ulp <= 1.0}
-            ok = ok and res['c3_segment_matmul']['pass']
-            del y_ref
+    ref = golden('bench_c2')
+    saved = torch.get_rng_state()
+    torch.manual_seed(777)
+    cmp = [compare_homo_golden(P.sampler.neighbor_sample(rowptr, col, s.to(dev), FANOUT), c) for s, c in zip(seeds, ref['calls'])]
+    rng_ok = digest(rng_prefix()) == ref['rng_after']
+    torch.set_rng_state(saved)
+    res['c2_neighbor_sample'] = {'against': 'reference (stored digests)', 'calls': len(cmp), 'edges': sum(c['edges'] for c in cmp),
+                                 'bit_exact': all(c['bit_exact'] for c in cmp), 'generator_state_equal': rng_ok,
+                                 'mismatch': sum((c['mismatch'] for c in cmp), [])}
+    ok = res['c2_neighbor_sample']['bit_exact'] and rng_ok
+    if with_matmul:
+        Nn, K, M, B = 1 << 20, 128, 128, 64
+        g = torch.Generator().manual_seed(0)
+        x = torch.randn(Nn, K, generator=g).to(torch.bfloat16)
+        w = (torch.randn(B, K, M, generator=g) / K ** 0.5).to(torch.bfloat16)
+        ptr = ragged_ptr(Nn, B, 100)
+        rows, y_ref = golden_rows('c3')
+        y = P.ops.segment_matmul(x.to(dev), ptr.to(dev), w.to(dev))[rows.to(dev)].cpu()
+        seg = torch.searchsorted(ptr, rows, right=True) - 1
+        tol = (x[rows].float().abs().unsqueeze(1) @ w[seg].float().abs()).squeeze(1) * (2.0 * K * 2.0 ** -24)
+        rel = float((y.float() - y_ref.float()).norm() / y_ref.float().norm())
+        ulp = lowp_ulp_excess(y, y_ref, tol)
+        res['c3_segment_matmul'] = {'against': 'reference (stored rows)', 'rows': int(rows.numel()), 'rel_frobenius': rel, 'max_ulp': ulp,
+                                    'tolerance': '<= 1e-3 and <= 1 bf16 ulp (+ the fp32 summation-order bound 2K 2^-24 |x||w| for cancelling results)',
+                                    'pass': rel <= 1e-3 and ulp <= 1.0}
+        ok = ok and res['c3_segment_matmul']['pass']
     res['pass'] = bool(ok)
     return res
 
@@ -320,25 +325,6 @@ def sampler_roofline(abi, step_dev, first, n_prof, torch, peaks, hbm_peak, peak_
             'kernel_ms_per_call': {k: v[0] / max(n_prof, 1) for k, v in prof.items() if v[1]}}
 
 
-def load_traffic():
-    """DRAM bytes per launch of the dominant kernels from the committed `ncu --set full` captures (profiles/)."""
-    out = {}
-    for fn in ('ncu_summary_r2.json', 'ncu_summary_r1.json'):
-        try:
-            summ = json.load(open(osp.join(ROOT, 'profiles', fn)))
-        except Exception:  # noqa
-            continue
-        for grp in summ.values():
-            for d in grp:
-                for nm in ('k_v2_sample', 'k_sample_s', 'k_sample', 'k_segment_matmul_tc'):
-                    if nm in d['Kernel Name']:
-                        out.setdefault(nm, []).append(1e6 * (float(d['dram__bytes_read.sum']) + float(d['dram__bytes_write.sum'])))
-                        break
-        if out:
-            break
-    return {k: sum(v) / len(v) for k, v in out.items()}
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
@@ -349,6 +335,8 @@ def main():
     ap.add_argument('--no-matmul', action='store_true')
     ap.add_argument('--no-parity', action='store_true')
     ap.add_argument('--no-c5', action='store_true', help='N=1: skip the papers100M-shaped single-GPU leg')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the last timed step\'s outputs (and a seeded sample of the segment_matmul result) as DIR/<name>.npy')
     a = ap.parse_args()
     a.warmup = max(a.warmup, 3)
     if a.impl == 'reference':
@@ -371,9 +359,10 @@ def main():
         peaks = json.load(open(osp.join(ROOT, 'MEASURED_PEAKS.json')))
     except Exception:  # noqa
         pass
-    hbm_peak = float(peaks.get('hbm_gbs', 6650.0))
-    peak_src = 'measured (MEASURED_PEAKS.json)' if 'hbm_gbs' in peaks else 'fallback 6.65 TB/s (B200_PROFILING.md)'
-    traffic = load_traffic()
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 — ceilings, not reached figures
+    hbm_peak = float(peaks.get('hbm_gbs', 3350.0))
+    peak_src = 'measured (MEASURED_PEAKS.json)' if 'hbm_gbs' in peaks else 'H100 SXM data sheet, 3.35 TB/s'
+    traffic = {}   # DRAM bytes per launch would come from a profiler capture; none is stored with the project
     mon = ClockMonitor(local).start()
     T = Timer(torch, dist, dev, world, mon, P)
 
@@ -388,7 +377,7 @@ def main():
         # ================================================================ N = 1: configs[1] (+ configs[2], configs[4] on one GPU)
         parity = None
         if not a.no_parity:
-            parity = parity_gates(P, dev, rowptr_c, col_c, rowptr, col, perm, with_matmul=not a.no_matmul)
+            parity = parity_gates(P, dev, rowptr, col, perm, with_matmul=not a.no_matmul)
             if not parity['pass']:
                 print(json.dumps({'metric': 'sampled_edges_per_s', 'value': None, 'parity': parity,
                                   'error': 'parity gate failed: nothing was timed'}), flush=True)
@@ -399,11 +388,17 @@ def main():
         seeds_host = [perm[b * BATCH:(b + 1) * BATCH].clone().pin_memory() for b in my_batches]
         seeds_dev = [s.to(dev) for s in seeds_host]
         torch.manual_seed(12345)
+        last = {}
 
         def step_dev(i):
-            return P.sampler.neighbor_sample(rowptr, col, seeds_dev[i], FANOUT)[0].numel()
+            out = P.sampler.neighbor_sample(rowptr, col, seeds_dev[i], FANOUT)
+            if a.dump_outputs and i == a.warmup + a.steps - 1:   # the last timed step
+                last['out'] = out
+            return out[0].numel()
         ms, edges, _, launches, clocks = T.run(step_dev, a.steps, a.warmup)
         value = edges / (ms * 1e-3)
+        if a.dump_outputs:
+            dump_sampler(a.dump_outputs, last.pop('out'))
 
         # e2e: pinned seeds -> device and (row, col, edge_id, node_id) -> pinned host EVERY step, through the public API.  The
         # calls themselves cannot overlap (each consumes the CPU generator where the previous one left it, and returns its
@@ -481,6 +476,7 @@ def main():
         if parity is not None:
             line['parity'] = parity
         rf = sampler_roofline(abi, step_dev, a.warmup, min(50, a.steps), torch, peaks, hbm_peak, peak_src, None)
+        last.clear()
         rf['traffic'] = traffic.get(rf['kernel'] + '_s') or traffic.get(rf['kernel'])
         rf['kernel'] += '_s'   # C2 runs the latency-path kernels (k_sample_s, ...)
         rf['note'] = 'C2 is latency-bound (~5 MB per call): the HBM fraction is reported, the binding limit is the ' \
@@ -498,30 +494,33 @@ def main():
             for _ in range(5):
                 y = P.ops.segment_matmul(x, ptr, w)
             torch.cuda.synchronize()
-            iters = 50
+            iters = min(a.steps, 50)
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             for _ in range(iters):
                 y = P.ops.segment_matmul(x, ptr, w)
             e1.record(); torch.cuda.synchronize()
             mm_ms = e0.elapsed_time(e1) / iters
+            if a.dump_outputs:
+                dump_matmul(a.dump_outputs, y)
             # e2e: features from pinned host memory in, result back to pinned host memory, every call
             yh = torch.empty(Nn, M, dtype=torch.bfloat16).pin_memory()
             for _ in range(2):
                 yh.copy_(P.ops.segment_matmul(xh.to(dev, non_blocking=True), ptr, w), non_blocking=True)
             torch.cuda.synchronize()
             e0.record()
-            for _ in range(10):
+            e2e_iters = min(a.steps, 10)
+            for _ in range(e2e_iters):
                 yh.copy_(P.ops.segment_matmul(xh.to(dev, non_blocking=True), ptr, w), non_blocking=True)
             e1.record(); torch.cuda.synchronize()
-            mm_e2e_ms = e0.elapsed_time(e1) / 10
+            mm_e2e_ms = e0.elapsed_time(e1) / e2e_iters
             flops, byts = 2.0 * Nn * K * M, Nn * K * 2 + Nn * M * 2 + B * K * M * 2 + (B + 1) * 8
-            tf_peak = float(peaks.get('bf16_tflops', 1590.0))
+            tf_peak = float(peaks.get('bf16_tflops', 989.0))
             line['segment_matmul'] = {
                 'config': '64 relations, N=2^20 ragged rows (log-normal lengths, one empty), 128->128 bf16, ptr on device',
                 'ms': mm_ms, 'tflops': flops / (mm_ms * 1e-3) / 1e12, 'algorithmic_bytes': byts,
                 'roofline': {'bound': 'hbm', 'achieved': byts / (mm_ms * 1e-3) / 1e9, 'peak': hbm_peak, 'unit': 'GB/s',
-                             'frac': byts / (mm_ms * 1e-3) / 1e9 / hbm_peak, 'traffic': traffic.get('k_segment_matmul_tc'),
+                             'frac': byts / (mm_ms * 1e-3) / 1e9 / hbm_peak, 'traffic': traffic.get('k_grouped_wgmma'),
                              'tensor_frac_of_bf16_peak': flops / (mm_ms * 1e-3) / 1e12 / tf_peak},
                 'e2e': {'value': flops / (mm_e2e_ms * 1e-3) / 1e12, 'unit': 'TFLOP/s', 'ms': mm_e2e_ms,
                         'h2d_bytes_per_step': Nn * K * 2, 'd2h_bytes_per_step': Nn * M * 2,
@@ -609,6 +608,26 @@ def main():
     mon.stop()
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_sampler(d, out):
+    """The arrays a caller of the timed neighbor_sample step receives, from its last step."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, t in zip(('row', 'col', 'node_id', 'edge_id'), out[:4]):
+        np.save(osp.join(d, f'neighbor_sample_{name}.npy'), t.cpu().numpy().astype(np.float64))
+    np.save(osp.join(d, 'neighbor_sample_nodes_per_hop.npy'), np.asarray(out[4], dtype=np.float64))
+    np.save(osp.join(d, 'neighbor_sample_edges_per_hop.npy'), np.asarray(out[5], dtype=np.float64))
+
+
+def dump_matmul(d, y, n_rows=16384):
+    """A fixed, seeded sample of rows of the last segment_matmul result (the full one is 256 MiB)."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    rows = torch.randperm(y.size(0), generator=torch.Generator().manual_seed(0))[:n_rows].sort().values
+    np.save(osp.join(d, 'segment_matmul_rows.npy'), rows.numpy().astype(np.float64))
+    np.save(osp.join(d, 'segment_matmul_out_sample.npy'), y[rows.to(y.device)].float().cpu().numpy())
 
 
 def c5_leg(a, P, abi, T, torch, dev, world, rank, peaks, hbm_peak, peak_src, traffic, dist):

@@ -1,5 +1,5 @@
 /*
- * include/pyg_b200.h — C ABI of libpyg_b200.so: the B200 (sm_100a) implementation of pyg-lib's two
+ * include/pyg_b200.h — C ABI of libpyg_b200.so: the H100 (sm_90a) implementation of pyg-lib's two
  * data-parallel hot paths.  Plain pointers and sizes only; no torch types.  Everything that is a
  * "const void* / void*" tensor argument is DEVICE memory on the current CUDA device unless it says
  * "host".  `stream` is a cudaStream_t passed as void*.
@@ -36,7 +36,7 @@ extern "C" {
 #define PYGB200_MM_ALLOW_TF32 1u  /* fp32 inputs may use TF32 tensor-core math
                                      (== torch.get_float32_matmul_precision() != 'highest',
                                      pyg_lib/csrc/ops/cuda/matmul_kernel.cu:159-165) */
-#define PYGB200_MM_FORCE_SIMT 2u  /* debugging: never take the tcgen05 path */
+#define PYGB200_MM_FORCE_SIMT 2u  /* debugging: never take the tensor-core paths */
 
 /* flags for the sampler entry points */
 #define PYGB200_S_REPLACE 1u
@@ -77,7 +77,7 @@ int64_t pygb200_timeline_read(uint64_t* out, int64_t cap);
  *   x [N,K], w [B,K,M], out [N,M] of `dtype`; ptr_dev [B+1] int64 on the DEVICE.
  * Replaces segment_matmul_kernel / grouped_matmul_out_kernel / run_grouped_gemm
  * (pyg_lib/csrc/ops/cuda/matmul_kernel.cu:304-319,121-287,21-100; CUTLASS 2.x sm80 GemmGrouped)
- * with a persistent sm_100a kernel: TMA-staged tiles -> tcgen05.mma -> TMEM -> epilogue.
+ * with a persistent sm_90a kernel: TMA-staged tiles -> wgmma (register accumulators) -> epilogue.
  * bias (optional, [B,M], may be NULL) is fused into the epilogue — it replaces the Python loop of
  * pyg_lib/ops/__init__.py:169-171.
  */

@@ -1,7 +1,7 @@
-"""Drop-in alias: `import pyg_lib` resolves to the B200 package so PyG finds
+"""Drop-in alias: `import pyg_lib` resolves to the pyg_lib_b200 package so PyG finds
 `pyg_lib.ops.segment_matmul`, `pyg_lib.sampler.neighbor_sample`, ... unchanged.
 
-The B200 package implements the CUDA path only (no CPU kernels: CPU tensors raise a clear RuntimeError).
+That package implements the CUDA path only (no CPU kernels: CPU tensors raise a clear RuntimeError).
 A deployment that also samples on the CPU (e.g. NeighborLoader worker processes over a host-resident graph)
 keeps the stock pyg-lib for that and opts out of this alias with PYG_LIB_B200_NO_ALIAS=1, importing
 `pyg_lib_b200` explicitly where the CUDA path is wanted."""

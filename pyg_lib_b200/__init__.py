@@ -1,4 +1,4 @@
-"""pyg_lib_b200 — B200-native drop-in for pyg-lib's two data-parallel hot paths
+"""pyg_lib_b200 — H100-native (sm_90a) drop-in for pyg-lib's two data-parallel hot paths
 (`pyg_lib.ops.segment_matmul/grouped_matmul`, `pyg_lib.sampler.neighbor_sample/hetero_neighbor_sample`).
 
 Mirrors the reference loader (pyg_lib/__init__.py:17-49): find `libpyg*.so` next to the package and

@@ -1,6 +1,6 @@
 """In-tree build of the two shared libraries (no cmake, no JIT cache):
 
-  pyg_lib_b200/libpyg_b200.so   CUDA kernels + C ABI (include/pyg_b200.h), nvcc -> sm_100a only
+  pyg_lib_b200/libpyg_b200.so   CUDA kernels + C ABI (include/pyg_b200.h), nvcc -> sm_90a (H100) only
   pyg_lib_b200/libpyg.so        torch dispatcher registration (pyg:: schemas) -> calls the C ABI
 
 `python -m pyg_lib_b200.build` or `__graft_entry__.build()`.  nvcc cross-compiles without a GPU.
@@ -20,11 +20,11 @@ CUDA_HOME = os.environ.get('CUDA_HOME', '/usr/local/cuda')
 NVCC = osp.join(CUDA_HOME, 'bin', 'nvcc')
 CXX = '/usr/bin/g++' if osp.exists('/usr/bin/g++') else 'g++'
 
-CU_SOURCES = ['sampler.cu', 'subgraph.cu', 'matmul.cu', 'matmul_tcgen05.cu', 'matmul_grouped_tc.cu']
+CU_SOURCES = ['sampler.cu', 'subgraph.cu', 'matmul.cu', 'matmul_grouped_tc.cu']
 TORCH_SOURCES = ['torch/library.cpp', 'torch/sampler_op.cpp', 'torch/subgraph_op.cpp', 'torch/matmul_op.cpp', 'torch/api.cpp']
-HEADERS = ['common.cuh', 'mt19937.cuh', 'sampler_v2.cuh', 'sampler_weighted.cuh', 'topk_replay.h', 'mkl_logf_table.inc', 'tcgen05_ptx.cuh', 'torch/common.h', 'torch/api.h', '../../include/pyg_b200.h']
+HEADERS = ['common.cuh', 'mt19937.cuh', 'sampler_v2.cuh', 'sampler_weighted.cuh', 'topk_replay.h', 'mkl_logf_table.inc', 'hopper_ptx.cuh', 'torch/common.h', 'torch/api.h', '../../include/pyg_b200.h']
 
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '--expt-relaxed-constexpr', '-Xcompiler', '-fPIC', '-ccbin', CXX, '-I' + osp.join(ROOT, 'include'),
               '-I' + CSRC]
 

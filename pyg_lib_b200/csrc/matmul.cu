@@ -8,9 +8,9 @@
 //     segments load-balance by tiles, and long reductions (the weight gradient dW[b] = X_b^T dY_b, whose
 //     K is the segment length) are split over K chunks that accumulate with fp32 atomics;
 //   * bf16 / fp16 / fp32 storage with fp32 FMA accumulation; optional fused bias.
-// The bf16/fp16 fast path for TMA-aligned segment_matmul lives in matmul_tcgen05.cu; this file is the
-// path for fp32 ('highest' precision == the reference's SIMT kernels, matmul_kernel.cu:227-282),
-// odd shapes, transposed views (grouped_matmul backward) and the weight gradient.
+// The tensor-core paths (bf16 / fp16, TF32, and the weight gradient for TMA-aligned shapes) live in
+// matmul_grouped_tc.cu; this file is the path for fp32 ('highest' precision == the reference's SIMT kernels,
+// matmul_kernel.cu:227-282) and for shapes or strides TMA cannot read.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -21,21 +21,18 @@
 
 namespace pygb200 {
 
-int segment_matmul_tcgen05(const void* x, const i64* ptr_dev, const void* w, const void* bias, void* out, i64 N, i64 K,
-                           i64 M, i64 B, int dtype, cudaStream_t st);  // matmul_tcgen05.cu
-bool tcgen05_supported(i64 N, i64 K, i64 M, i64 B, int dtype, const void* x, const void* w, const void* out);
-int segment_wgrad_tcgen05(const void* x, const i64* ptr_dev, const void* dy, void* dw, i64 N, i64 K, i64 M, i64 B, int dtype,
-                          cudaStream_t st);
-bool wgrad_tcgen05_supported(i64 N, i64 K, i64 M, i64 B, int dtype, const void* x, const void* dy, const void* dw);
+// matmul_grouped_tc.cu: the Hopper tensor-core (wgmma) grouped GEMM behind every bf16 / fp16 / TF32 path
+bool segment_tc_supported(i64 N, i64 K, i64 M, i64 B, int dtype, const void* x, const void* w, const void* out);
+int segment_matmul_tc(const void* x, const i64* ptr_dev, const void* w, const void* bias, void* out, i64 N, i64 K, i64 M, i64 B,
+                      int dtype, cudaStream_t st);
+bool tf32_supported(i64 N, i64 K, i64 M, i64 B, const void* x, const void* w, const void* out);
 int segment_matmul_tf32(const void* x, const i64* ptr_dev, const void* w, const void* bias, void* out, i64 N, i64 K, i64 M,
                         i64 B, cudaStream_t st);
-bool tf32_supported(i64 N, i64 K, i64 M, i64 B, const void* x, const void* w, const void* out);
-// matmul_grouped_tc.cu: general tensor-core grouped GEMM (any K / M multiple of 8, transposed views, many problems)
+bool wgrad_tc_supported(i64 N, i64 K, i64 M, i64 B, int dtype, const void* x, const void* dy, const void* dw);
+int segment_wgrad_tc(const void* x, const i64* ptr_dev, const void* dy, void* dw, i64 N, i64 K, i64 M, i64 B, int dtype,
+                     cudaStream_t st);
 bool grouped_tc_supported(const pygb200_gemm_problem* ps, i64 count, int dtype);
 int grouped_matmul_tc(const pygb200_gemm_problem* ps, i64 count, int dtype, cudaStream_t st);
-bool segment_tc_general_supported(i64 N, i64 K, i64 M, i64 B, int dtype, const void* x, const void* w, const void* out);
-int segment_matmul_tc_general(const void* x, const i64* ptr_dev, const void* w, const void* bias, void* out, i64 N, i64 K, i64 M,
-                              i64 B, int dtype, cudaStream_t st);
 
 // "invalid ptr" flag of the segment kernels: one int in pinned, mapped, portable host memory.  The kernels validate
 // `ptr` while they read it (ptr[0] == 0, non-decreasing, ptr[B] == N — what the reference's split_with_sizes checks on
@@ -92,7 +89,7 @@ __host__ __device__ inline i64 work_items(i64 n, i64 m, i64 k, i64 kchunk) {
 // problems[b] for segment b of a segment_matmul; also the flat work-item prefix (single block).
 //   mode 0: forward   C_b = X[ptr_b:ptr_b+1] @ W[b]            (n=len, k=K, m=M)
 //   mode 1: wgrad     dW[b] = X_b^T @ dY_b                      (n=K, k=len, m=M), split over K chunks
-__global__ void k_build_segments(Problem* probs, i64* total_tiles, const i64* __restrict__ ptr, const char* x,
+__global__ void __launch_bounds__(1024) k_build_segments(Problem* probs, i64* total_tiles, const i64* __restrict__ ptr, const char* x,
                                  const char* w, const char* bias, char* out, float* acc, i64 K, i64 M, i64 B, int esize,
                                  int mode, i64 N, int* err, i64 wgrad_kchunk) {
   __shared__ i64 s_carry;
@@ -272,7 +269,7 @@ __global__ void k_finish_split(const Problem* __restrict__ probs, i64 P) {
 }
 
 int launch_grouped(const Problem* probs_dev, i64 P, const i64* total_dev, i64 tiles_bound, int dtype, cudaStream_t st) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   i64 g = tiles_bound < 1 ? 1 : tiles_bound;
@@ -371,14 +368,12 @@ extern "C" int pygb200_segment_matmul(const void* x, const int64_t* ptr_dev, con
   }
   if (K == 0)   // empty contraction: every row of segment b is bias[b] (the generic kernel runs zero K steps and adds the bias)
     return segment_generic(x, (const i64*)ptr_dev, w, bias, out, N, K, M, B, dtype, 0, st);
-  if (!(flags & PYGB200_MM_FORCE_SIMT) && tcgen05_supported(N, K, M, B, dtype, x, w, out))
-    return segment_matmul_tcgen05(x, (const i64*)ptr_dev, w, bias, out, N, K, M, B, dtype, st);
   if (!(flags & PYGB200_MM_FORCE_SIMT) && (flags & PYGB200_MM_ALLOW_TF32) && dtype == PYGB200_F32 &&
       tf32_supported(N, K, M, B, x, w, out))
     return segment_matmul_tf32(x, (const i64*)ptr_dev, w, bias, out, N, K, M, B, st);
-  if (!(flags & PYGB200_MM_FORCE_SIMT) && segment_tc_general_supported(N, K, M, B, dtype, x, w, out)) {
+  if (!(flags & PYGB200_MM_FORCE_SIMT) && segment_tc_supported(N, K, M, B, dtype, x, w, out)) {
     keep_pool_memory();
-    return segment_matmul_tc_general(x, (const i64*)ptr_dev, w, bias, out, N, K, M, B, dtype, st);
+    return segment_matmul_tc(x, (const i64*)ptr_dev, w, bias, out, N, K, M, B, dtype, st);
   }
   return segment_generic(x, (const i64*)ptr_dev, w, bias, out, N, K, M, B, dtype, 0, st);
 }
@@ -394,8 +389,8 @@ extern "C" int pygb200_segment_matmul_wgrad(const void* x, const int64_t* ptr_de
   PYGB_CHECK(!mm_take_async_error(), PYGB200_ERR_ARG,
              "segment_matmul_wgrad: an EARLIER segment_matmul / wgrad call received an invalid ptr; that call's output is undefined");
   keep_pool_memory();
-  if (!(flags & PYGB200_MM_FORCE_SIMT) && N > 0 && wgrad_tcgen05_supported(N, K, M, B, dtype, x, dy, dw))
-    return segment_wgrad_tcgen05(x, (const i64*)ptr_dev, dy, dw, N, K, M, B, dtype, (cudaStream_t)stream);
+  if (!(flags & PYGB200_MM_FORCE_SIMT) && N > 0 && wgrad_tc_supported(N, K, M, B, dtype, x, dy, dw))
+    return segment_wgrad_tc(x, (const i64*)ptr_dev, dy, dw, N, K, M, B, dtype, (cudaStream_t)stream);
   // empty segments produce zero gradients: their single work item runs the k-loop zero times and stores 0
   return segment_generic(x, (const i64*)ptr_dev, dy, nullptr, dw, N, K, M, B, dtype, 1, (cudaStream_t)stream);
 }

@@ -1,21 +1,25 @@
-// pyg_lib_b200/csrc/matmul_grouped_tc.cu — general grouped GEMM on Blackwell tensor cores (bf16 / fp16).
+// pyg_lib_b200/csrc/matmul_grouped_tc.cu — grouped GEMM on Hopper tensor cores (wgmma + TMA + mbarrier, sm_90a).
 //
 // Replaces the reference's TensorOp grouped GEMM (pyg_lib/csrc/ops/cuda/matmul_kernel.cu:121-287: CUTLASS 2.x
-// GemmGrouped, any K / M) for everything the specialised segment kernel of matmul_tcgen05.cu does not take:
+// GemmGrouped, mma.sync) with one hand-written persistent kernel that serves every tensor-core matmul of the library:
+//   * pyg::segment_matmul in bf16 / fp16 (any K, M that are multiples of 8 elements — the TMA row-pitch rule) and in
+//     fp32 storage with TF32 math when the caller allows it; the problem list is built ON THE DEVICE from `ptr`, so a
+//     device-resident `ptr` costs no host sync;
 //   * pyg::grouped_matmul (matmul_kernel.cu:289-302) — independent problems C_i = A_i @ B_i, including the transposed
-//     VIEWS its backward passes in (dX = dY @ W^T, dW = X^T @ dY): an operand stored transposed is simply the other
-//     UMMA major-ness (A MN-major / B K-major), selected per problem in the instruction descriptor — no copies;
-//   * pyg::segment_matmul with K or M outside {64,128,192,256} (any K, M that are multiples of 8 elements — the
-//     TMA row-pitch rule), any number of segments; the problem list is built ON THE DEVICE from `ptr`.
-// One persistent CTA per SM, 256 threads, warp-specialised like the segment kernel:
-//   warp 0 lane 0  TMA producer: per K step of 64 one stage = A tile [128 x 64] + B tile [64 x BN] (BN <= 256), 4-stage
-//                  mbarrier ring; out-of-range K / M / rows are zero-filled by TMA, so tails need no special cases;
-//   warp 1 lane 0  tcgen05.mma issuer (kind::f16, M = 128, N = BN rounded up to 16), accumulating over the K steps
-//                  into one of two TMEM accumulators;
-//   warp 2         TMEM allocator;   warps 4-7  epilogue: tcgen05.ld -> (+bias) -> bf16/fp16 -> predicated 16-byte
-//                  row stores (a thread owns one output row; 64 contiguous bytes per TMEM load).
-// Tiles of all problems form one flat list dealt round-robin to the CTAs.  Per-problem tensor maps live in global
-// memory (uploaded with the problem list; the producer fences them in with fence.proxy.tensormap::generic).
+//     VIEWS its backward passes in (dX = dY @ W^T, dW = X^T @ dY): an operand stored transposed is consumed MN-major
+//     through wgmma's transpose bit — no copies;
+//   * the weight gradient dW[b] = X_b^T dY_b of segment_matmul (contraction over the rows of a segment).
+// One CTA per SM, 384 threads:
+//   warpgroup 0, one thread   TMA producer: per K step one stage = A tile [128 rows x 128 bytes of K] + B tile
+//                             [128 bytes of K x 128 columns], 4-stage mbarrier ring, SWIZZLE_128B; out-of-range K / M /
+//                             rows are zero-filled by TMA, so tails need no special cases;
+//   warpgroups 1, 2           wgmma m64n128 (k16 for 16-bit, k8 for TF32) on rows [0, 64) / [64, 128) of the tile,
+//                             fp32 accumulators in registers; epilogue: registers -> fp32 staging tile in shared memory
+//                             -> (+bias) -> storage type -> coalesced 16-byte row stores, predicated on the tails.
+// Tiles of all problems form one flat list dealt round-robin to the CTAs (column tiles of one row tile are adjacent, so
+// their A loads meet in L2).  Long contractions with few output tiles are split over K chunks whose fp32 partials are
+// added in chunk order by k_gt_finish (bit-reproducible, no atomics).
+// H100: 132 SMs, up to 227 KB of shared memory per block — the 4 x 32 KB ring plus 2 x 33 KB staging tiles fit one CTA.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -31,44 +35,39 @@ namespace pygb200 {
 int* mm_error_flag_dev();   // matmul.cu
 namespace {
 
-#include "tcgen05_ptx.cuh"
+#include "hopper_ptx.cuh"
 
-constexpr int GT_TM = 128;       // rows per tile == UMMA M
-constexpr int GT_BN = 256;       // max columns per tile == max UMMA N (two accumulators fill the 512 TMEM columns)
-constexpr int GT_BK = 64;        // K elements per stage == one 128-byte swizzle row
+constexpr int GT_TM = 128;       // rows per tile: two consumer warpgroups x wgmma M = 64
+constexpr int GT_BN = 128;       // columns per tile == wgmma N
 constexpr int GT_STAGES = 4;
-constexpr int GT_NT = 256;
-constexpr u32 GT_A_BYTES = GT_TM * GT_BK * 2;            // 16 KB
-constexpr u32 GT_B_GROUP = 64 * GT_BK * 2;               // 8 KB per 64 columns of B
-constexpr u32 GT_STAGE_BYTES = GT_A_BYTES + (GT_BN / 64) * GT_B_GROUP;   // 48 KB
+constexpr int GT_NT = 384;
+constexpr u32 GT_A_BYTES = GT_TM * 128;                    // 16 KB: 128 rows x one 128-byte swizzle row of K
+constexpr u32 GT_STAGE_BYTES = GT_A_BYTES + GT_BN * 128;   // 32 KB
+constexpr int GT_SP = GT_BN + 4;                           // fp32 staging pitch (floats)
+constexpr u32 GT_OUT_BYTES = 64 * GT_SP * 4;               // one consumer warpgroup's staging tile
+constexpr int MAX_SEG = 1024;                              // segments of the TF32 / weight-gradient paths
+
+// element kinds of the kernel
+constexpr int ET_F16 = 0, ET_BF16 = 1, ET_TF32 = 2;
 
 struct GProb {
   const CUtensorMap* map_a;    // K-major A: dims [k, rows]; MN-major A (transposed view): dims [n, k]
   const CUtensorMap* map_b;    // MN-major B: dims [m, k, z]; K-major B (transposed view): dims [k, m, z]
-  unsigned char* c;            // row-major output of this problem
-  const unsigned char* bias;   // [m] or null
+  unsigned char* c;            // row-major output of this problem (storage type; fp32 when c_f32)
+  const unsigned char* bias;   // [m] or null (storage type of c)
   i64 ldc;                     // elements
   int n, k, m;
-  int a_row0;                  // K-major A: row offset of this problem inside map_a (segment mode)
+  int a_off;                   // K-major A: row of this problem's first row in map_a; MN-major A: its first k
+  int b_k0;                    // first k of this problem in map_b
   int b_z;                     // third coordinate into map_b (segment index)
   int a_mn, b_k;               // operand stored transposed
   int c_vec;                   // rows of C are 16-byte aligned
+  int c_f32;                   // fp32 output (TF32 kernel)
+  int zero_ktail;              // k past `k` in the last stage are rows of the next segment: zero them in shared memory
   int tile0, tiles_n;          // first flat tile of the problem; number of column tiles
-  int ksplit, ksteps_chunk;    // split-K: number of K chunks (1 = none) and K steps (of 64) per chunk
-  float* part;                 // split-K: [ksplit][n, m] fp32 partial products, added in chunk order by k_gt_finish
+  int ksplit, ksteps_chunk;    // K chunks (work items per output tile) and K steps per chunk
+  float* part;                 // non-null: [ksplit][n, m] fp32 partial products, added in chunk order by k_gt_finish
 };
-
-__device__ __forceinline__ void tma_load_3d(u32 dst, const CUtensorMap* map, int c0, int c1, int c2, u32 bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];" ::"r"(dst),
-      "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(bar)
-      : "memory");
-}
-// a tensor map that was written to global memory through the generic proxy (the host's copy) must be fenced
-// into the tensormap proxy before the TMA unit reads it
-__device__ __forceinline__ void fence_tensormap(const CUtensorMap* map) {
-  asm volatile("fence.proxy.tensormap::generic.acquire.sys [%0], 128;" ::"l"(map) : "memory");
-}
 
 struct TileRef { int p, i, j, kc; };
 __device__ __forceinline__ TileRef find_tile(const GProb* __restrict__ probs, int P, int t) {
@@ -82,176 +81,199 @@ __device__ __forceinline__ TileRef find_tile(const GProb* __restrict__ probs, in
   return {lo, mn / tn, mn % tn, local / (tm * tn)};
 }
 
-template <bool BF16>
-__global__ void __launch_bounds__(GT_NT, 1) k_grouped_tc(const GProb* __restrict__ probs, int P, const int* __restrict__ total_ptr) {
+// the four wgmma of one stage (K = 64 16-bit or 32 TF32 elements) for consumer warpgroup `c`
+template <int ET, int TA, int TB>
+__device__ __forceinline__ void mma_stage(float (&d)[64], u32 a_base, u32 b_base, int c) {
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    // K-major: 32 bytes per K step inside the 128-byte swizzle row; MN-major: 16 K rows = 2 KB per step, 64-wide groups
+    const u64 da = TA ? make_desc(a_base + c * 8192 + kk * 2048, 8192, 1024) : make_desc(a_base + c * 8192 + kk * 32, 16, 1024);
+    const u64 db = TB ? make_desc(b_base + kk * 2048, 8192, 1024) : make_desc(b_base + kk * 32, 16, 1024);
+    if constexpr (ET == ET_TF32) wgmma_tf32(d, da, db);
+    else wgmma_16<ET == ET_BF16, TA, TB>(d, da, db);
+  }
+}
+
+// LAYOUT: operand major-ness, per problem at run time (LAY_ANY: grouped_matmul) or fixed for the whole launch (segment
+// paths) — a fixed one keeps the wgmma of a stage free of branches, so ptxas does not serialise them
+constexpr int LAY_ANY = 0, LAY_FWD = 1, LAY_WGRAD = 2;
+
+template <int ET, int LAYOUT>
+__global__ void __launch_bounds__(GT_NT, 1) k_grouped_wgmma(const GProb* __restrict__ probs, int P, const int* __restrict__ total_ptr) {
+  constexpr int BK = ET == ET_TF32 ? 32 : 64;   // K elements per stage: one 128-byte swizzle row
   extern __shared__ unsigned char smem_raw[];
   const u32 raw = smem_u32(smem_raw);
   const u32 base = (raw + 1023u) & ~1023u;
   unsigned char* sm = smem_raw + (base - raw);
-  const u32 off_bar = GT_STAGES * GT_STAGE_BYTES;
+  const u32 off_out = GT_STAGES * GT_STAGE_BYTES, off_bar = off_out + 2 * GT_OUT_BYTES;
   const u32 bar0 = base + off_bar;
   auto FULL = [&](int s) { return bar0 + 8u * (u32)s; };
   auto EMPTY = [&](int s) { return bar0 + 8u * (u32)(GT_STAGES + s); };
-  auto T_FULL = [&](int s) { return bar0 + 8u * (u32)(2 * GT_STAGES + s); };
-  auto T_EMPTY = [&](int s) { return bar0 + 8u * (u32)(2 * GT_STAGES + 2 + s); };
-  constexpr int NBARS = 2 * GT_STAGES + 4;
-  u32* tmem_slot = reinterpret_cast<u32*>(sm + off_bar + NBARS * 8);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
 
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < GT_STAGES; ++s) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(T_FULL(s), 1); mbar_init(T_EMPTY(s), 128); }
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < GT_STAGES; ++s) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    fence_proxy_async();
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const u32 tmem_base = *tmem_slot;
   const int total = *total_ptr;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ================================ TMA producer ================================
-    if (lane == 0) {
-      int stage = 0, last_p = -1;
-      u32 phase = 0;
-      for (int t = blockIdx.x; t < total; t += gridDim.x) {
-        const TileRef tr = find_tile(probs, P, t);
-        const GProb& pb = probs[tr.p];
-        if (tr.p != last_p) { fence_tensormap(pb.map_a); fence_tensormap(pb.map_b); last_p = tr.p; }
-        const int cols = min(GT_BN, pb.m - tr.j * GT_BN), groups = (cols + 63) >> 6;
-        const int ks0 = tr.kc * pb.ksteps_chunk, ks1 = min((pb.k + GT_BK - 1) / GT_BK, ks0 + pb.ksteps_chunk);
-        for (int ks = ks0; ks < ks1; ++ks) {
-          mbar_wait(EMPTY(stage), phase ^ 1);
-          const u32 a_dst = base + stage * GT_STAGE_BYTES, b_dst = a_dst + GT_A_BYTES;
-          mbar_expect_tx(FULL(stage), GT_A_BYTES + groups * GT_B_GROUP);
-          if (!pb.a_mn) {   // box [64 k x 128 rows] -> [128][128 B]
-            tma_load_2d(a_dst, pb.map_a, ks * GT_BK, pb.a_row0 + tr.i * GT_TM, FULL(stage));
-          } else {          // two boxes [64 n x 64 k]: MN-major atoms, 8 KB per 64 rows of the tile
-            tma_load_2d(a_dst, pb.map_a, tr.i * GT_TM, ks * GT_BK, FULL(stage));
-            tma_load_2d(a_dst + 8192, pb.map_a, tr.i * GT_TM + 64, ks * GT_BK, FULL(stage));
-          }
-          for (int gq = 0; gq < groups; ++gq) {
-            if (!pb.b_k) tma_load_3d(b_dst + gq * GT_B_GROUP, pb.map_b, tr.j * GT_BN + gq * 64, ks * GT_BK, pb.b_z, FULL(stage));   // [64 k][128 B]
-            else tma_load_3d(b_dst + gq * GT_B_GROUP, pb.map_b, ks * GT_BK, tr.j * GT_BN + gq * 64, pb.b_z, FULL(stage));          // [64 cols][128 B]
-          }
-          if (++stage == GT_STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================================ MMA issuer ================================
-    int stage = 0, acc = 0;
-    u32 phase = 0, t_phase = 0;
-    const u32 fmt = BF16 ? 1u : 0u;
-    for (int t = blockIdx.x; t < total; t += gridDim.x) {
-      const TileRef tr = find_tile(probs, P, t);
+    if (t != 0) return;
+    int stage = 0, last_p = -1;
+    u32 phase = 0;
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+      const TileRef tr = find_tile(probs, P, tile);
       const GProb& pb = probs[tr.p];
-      const int cols = min(GT_BN, pb.m - tr.j * GT_BN);
-      const u32 un = (u32)((cols + 15) & ~15);   // UMMA N: multiple of 16 (columns past m are zero-filled B)
-      // D = f32 (bit 4), A/B format (bits 7-9 / 10-12), A major (bit 15), B major (bit 16; 1 = MN-major), N >> 3, M >> 4
-      const u32 idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((u32)(pb.a_mn ? 1 : 0) << 15) | ((u32)(pb.b_k ? 0 : 1) << 16) |
-                        ((un >> 3) << 17) | ((u32)(GT_TM >> 4) << 24);
-      const int ks0 = tr.kc * pb.ksteps_chunk, ksteps = min((pb.k + GT_BK - 1) / GT_BK, ks0 + pb.ksteps_chunk);
-      mbar_wait(T_EMPTY(acc), ((t_phase >> acc) & 1u) ^ 1u);
-      const u32 d_tmem = tmem_base + (u32)(acc * GT_BN);
-      for (int ks = ks0; ks < ksteps; ++ks) {
-        mbar_wait(FULL(stage), phase);
-        tc_fence_after();
-        if (lane == 0) {
-          const u32 a_base = base + stage * GT_STAGE_BYTES, b_base = a_base + GT_A_BYTES;
-          const int kk_n = min(4, (pb.k - ks * GT_BK + 15) >> 4);   // K = 16 per instruction; skip all-zero steps of the K tail
-          for (int kk = 0; kk < kk_n; ++kk) {
-            const u64 adesc = pb.a_mn ? make_desc(a_base + kk * 2048, 8192, 1024) : make_desc(a_base + kk * 32, 16, 1024);
-            const u64 bdesc = pb.b_k ? make_desc(b_base + kk * 32, 16, 1024) : make_desc(b_base + kk * 2048, GT_B_GROUP, 1024);
-            tc_mma_f16(d_tmem, adesc, bdesc, idesc, (ks > ks0 || kk > 0) ? 1u : 0u);
-          }
-          tc_commit(EMPTY(stage));
-          if (ks == ksteps - 1) tc_commit(T_FULL(acc));
+      if (tr.p != last_p) { fence_tensormap(pb.map_a); fence_tensormap(pb.map_b); last_p = tr.p; }
+      const int ks0 = tr.kc * pb.ksteps_chunk, ks1 = min((pb.k + BK - 1) / BK, ks0 + pb.ksteps_chunk);
+      for (int ks = ks0; ks < ks1; ++ks) {
+        mbar_wait(EMPTY(stage), phase ^ 1);
+        const u32 a_dst = base + stage * GT_STAGE_BYTES, b_dst = a_dst + GT_A_BYTES, full = FULL(stage);
+        const int k0 = ks * BK;
+        mbar_expect_tx(full, GT_STAGE_BYTES);   // (boxes partly or wholly out of range still deliver their full size)
+        if (!pb.a_mn) {   // box [BK x 128 rows] -> [128][128 B]
+          tma_load_2d(a_dst, pb.map_a, k0, pb.a_off + tr.i * GT_TM, full);
+        } else {          // two boxes [64 n x 64 k]: MN-major atoms, 8 KB per 64 rows of the tile
+          tma_load_2d(a_dst, pb.map_a, tr.i * GT_TM, pb.a_off + k0, full);
+          tma_load_2d(a_dst + 8192, pb.map_a, tr.i * GT_TM + 64, pb.a_off + k0, full);
         }
-        __syncwarp();
+        if (pb.b_k) {     // box [BK x 128 columns] -> [128][128 B]
+          tma_load_3d(b_dst, pb.map_b, pb.b_k0 + k0, tr.j * GT_BN, pb.b_z, full);
+        } else {          // two boxes [64 columns x 64 k]
+          tma_load_3d(b_dst, pb.map_b, tr.j * GT_BN, pb.b_k0 + k0, pb.b_z, full);
+          tma_load_3d(b_dst + 8192, pb.map_b, tr.j * GT_BN + 64, pb.b_k0 + k0, pb.b_z, full);
+        }
         if (++stage == GT_STAGES) { stage = 0; phase ^= 1; }
       }
-      t_phase ^= 1u << acc;
-      acc ^= 1;
     }
-  } else if (warp >= 4) {
-    // ================================ epilogue (128 threads) ================================
-    const int q = warp & 3, r = q * 32 + lane;
-    int acc = 0;
-    u32 t_phase = 0;
-    for (int t = blockIdx.x; t < total; t += gridDim.x) {
-      const TileRef tr = find_tile(probs, P, t);
-      const GProb& pb = probs[tr.p];
-      const int col0 = tr.j * GT_BN, cols = min(GT_BN, pb.m - col0);
-      const i64 grow = (i64)tr.i * GT_TM + r;
-      const bool row_ok = grow < pb.n;
-      unsigned char* crow = pb.c + (grow * pb.ldc + col0) * 2;
-      mbar_wait(T_FULL(acc), (t_phase >> acc) & 1u);
-      t_phase ^= 1u << acc;
-      tc_fence_after();
-      for (int c = 0; c < cols; c += 32) {
-        u32 v[32];
-        tc_ld_32x32(tmem_base + (u32)(acc * GT_BN + c) + ((u32)(q * 32) << 16), v);
-        tc_wait_ld();
-        if (!row_ok) continue;
-        const int nc = min(32, cols - c);
-        if (pb.ksplit > 1) {   // fp32 partial of this K chunk; bias / rounding happen in k_gt_finish
-          float* dst = pb.part + ((i64)tr.kc * pb.n + grow) * pb.m + col0 + c;
-          if (nc == 32 && (pb.m & 3) == 0) {
+    return;
+  }
+
+  // ================================ consumers: wgmma + epilogue ================================
+  const int c = wg - 1, warp = t >> 5, lane = t & 31;
+  float* stg = reinterpret_cast<float*>(sm + off_out + c * GT_OUT_BYTES);
+  int stage = 0;
+  u32 phase = 0;
+  for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+    const TileRef tr = find_tile(probs, P, tile);
+    const GProb& pb = probs[tr.p];
+    const int ks0 = tr.kc * pb.ksteps_chunk, ks1 = min((pb.k + BK - 1) / BK, ks0 + pb.ksteps_chunk);
+    float d[64];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) reinterpret_cast<uint4*>(dst)[j] = make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) if (j < nc) dst[j] = __uint_as_float(v[j]);
-          }
-          continue;
+    for (int i = 0; i < 64; ++i) d[i] = 0.f;
+    for (int ks = ks0; ks < ks1; ++ks) {
+      mbar_wait(FULL(stage), phase);
+      const u32 a_base = base + stage * GT_STAGE_BYTES, b_base = a_base + GT_A_BYTES;
+      if (ET != ET_TF32 && pb.zero_ktail && (ks + 1) * BK > pb.k) {
+        // rows [valid, 64) of the four [64 k][128 B] boxes (A and B are both MN-major here) belong to the next segment;
+        // a row is one 128-byte line whatever the swizzle
+        const int valid = pb.k - ks * BK, per_box = (BK - valid) * 8;
+        unsigned char* st = sm + stage * GT_STAGE_BYTES;
+        for (int q = threadIdx.x - 128; q < 4 * per_box; q += 256) {
+          const int box = q / per_box, rem = q - box * per_box;
+          *reinterpret_cast<uint4*>(st + box * 8192 + (valid + (rem >> 3)) * 128 + (rem & 7) * 16) = make_uint4(0, 0, 0, 0);
         }
-        if (pb.bias) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (j < nc) v[j] = __float_as_uint(__uint_as_float(v[j]) + ld_bias<BF16>(pb.bias, col0 + c + j));
-        }
-        if (nc == 32 && pb.c_vec) {
-          uint4* dst = reinterpret_cast<uint4*>(crow + c * 2);
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            dst[j] = make_uint4(pack2<BF16>(__uint_as_float(v[8 * j]), __uint_as_float(v[8 * j + 1])),
-                                pack2<BF16>(__uint_as_float(v[8 * j + 2]), __uint_as_float(v[8 * j + 3])),
-                                pack2<BF16>(__uint_as_float(v[8 * j + 4]), __uint_as_float(v[8 * j + 5])),
-                                pack2<BF16>(__uint_as_float(v[8 * j + 6]), __uint_as_float(v[8 * j + 7])));
+        fence_proxy_async();
+        named_bar(1, 256);
+      }
+      wg_fence();
+      if constexpr (ET == ET_TF32) {
+        mma_stage<ET, 0, 0>(d, a_base, b_base, c);
+      } else if constexpr (LAYOUT == LAY_FWD) {
+        mma_stage<ET, 0, 1>(d, a_base, b_base, c);
+      } else if constexpr (LAYOUT == LAY_WGRAD) {
+        mma_stage<ET, 1, 1>(d, a_base, b_base, c);
+      } else {
+        if (pb.a_mn) {
+          if (pb.b_k) mma_stage<ET, 1, 0>(d, a_base, b_base, c); else mma_stage<ET, 1, 1>(d, a_base, b_base, c);
         } else {
-          unsigned short* dst = reinterpret_cast<unsigned short*>(crow + c * 2);
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (j < nc) dst[j] = (unsigned short)(pack2<BF16>(__uint_as_float(v[j]), 0.f) & 0xffffu);
+          if (pb.b_k) mma_stage<ET, 0, 0>(d, a_base, b_base, c); else mma_stage<ET, 0, 1>(d, a_base, b_base, c);
         }
       }
-      tc_fence_before();
-      mbar_arrive(T_EMPTY(acc));
-      acc ^= 1;
+      wg_commit();
+      wg_wait_all();
+      if (t == 0) mbar_arrive(EMPTY(stage));   // this warpgroup's reads of the stage are done
+      if (++stage == GT_STAGES) { stage = 0; phase ^= 1; }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+
+    // fragment -> staging: thread holds rows warp*16 + lane/4 (+8), columns 8j + 2(lane%4) (+1)
+    named_bar(2 + c, 128);   // the previous tile's stores have finished reading the staging tile
+    {
+      const int r = warp * 16 + (lane >> 2), col = 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        *reinterpret_cast<float2*>(stg + r * GT_SP + 8 * j + col) = make_float2(d[4 * j], d[4 * j + 1]);
+        *reinterpret_cast<float2*>(stg + (r + 8) * GT_SP + 8 * j + col) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+      }
+    }
+    named_bar(2 + c, 128);
+    // staging -> global: 16-byte chunks, consecutive threads along a row
+    const int col0 = tr.j * GT_BN, cols = min(GT_BN, pb.m - col0);
+    const i64 row0 = (i64)tr.i * GT_TM + c * 64;
+    const int rows = (int)min((i64)64, (i64)pb.n - row0);
+    if (rows <= 0) continue;
+    if (pb.part != nullptr || ET == ET_TF32) {
+      // fp32 out: a split-K partial (no bias) or the TF32 kernel's result
+      const bool partial = pb.part != nullptr;
+      float* cb = partial ? pb.part + (i64)tr.kc * pb.n * pb.m : reinterpret_cast<float*>(pb.c);
+      const i64 ldc = partial ? (i64)pb.m : pb.ldc;
+      const bool vec = partial ? (pb.m & 3) == 0 : pb.c_vec != 0;
+      const float* bias = partial ? nullptr : reinterpret_cast<const float*>(pb.bias);
+      for (int q = t; q < rows * 32; q += 128) {
+        const int r = q >> 5, cc = (q & 31) * 4;
+        if (cc >= cols) continue;
+        const float4 v4 = *reinterpret_cast<const float4*>(stg + r * GT_SP + cc);
+        float e[4] = {v4.x, v4.y, v4.z, v4.w};
+        if (bias) {
+#pragma unroll
+          for (int u = 0; u < 4; ++u) if (cc + u < cols) e[u] += bias[col0 + cc + u];
+        }
+        float* dst = cb + (row0 + r) * ldc + col0 + cc;
+        if (vec && cc + 4 <= cols) {
+          *reinterpret_cast<float4*>(dst) = make_float4(e[0], e[1], e[2], e[3]);
+        } else {
+#pragma unroll
+          for (int u = 0; u < 4; ++u) if (cc + u < cols) dst[u] = e[u];
+        }
+      }
+    } else if constexpr (ET != ET_TF32) {
+      constexpr bool BF = ET == ET_BF16;
+      for (int q = t; q < rows * 16; q += 128) {
+        const int r = q >> 4, cc = (q & 15) * 8;
+        if (cc >= cols) continue;
+        const float4 v0 = *reinterpret_cast<const float4*>(stg + r * GT_SP + cc);
+        const float4 v1 = *reinterpret_cast<const float4*>(stg + r * GT_SP + cc + 4);
+        float e[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+        if (pb.bias) {
+#pragma unroll
+          for (int u = 0; u < 8; ++u) if (cc + u < cols) e[u] += ld_bias<BF>(pb.bias, col0 + cc + u);
+        }
+        unsigned short* dst = reinterpret_cast<unsigned short*>(pb.c) + (row0 + r) * pb.ldc + col0 + cc;
+        if (pb.c_vec && cc + 8 <= cols) {
+          *reinterpret_cast<uint4*>(dst) = make_uint4(pack2<BF>(e[0], e[1]), pack2<BF>(e[2], e[3]), pack2<BF>(e[4], e[5]), pack2<BF>(e[6], e[7]));
+        } else {
+#pragma unroll
+          for (int u = 0; u < 8; ++u) if (cc + u < cols) dst[u] = (unsigned short)(pack2<BF>(e[u], 0.f) & 0xffffu);
+        }
+      }
+    }
   }
 }
 
-// segment mode: problems[b] for segment b of a segment_matmul (all share map_a / map_b), flat tile prefix; one block
-__global__ void k_gt_build_segments(GProb* probs, int* total, const i64* __restrict__ ptr, const CUtensorMap* map_a,
+// segment mode: problems[b] for segment b (all share map_a / map_b), flat tile prefix; one block.
+//   mode 0 (forward)  C_b = X[ptr_b:ptr_b+1] @ W[b]  (n = len, k = K, m = M); W enters MN-major ([K, M] per segment) or,
+//                      for TF32, K-major ([M, K] per segment, b_k = 1)
+//   mode 1 (wgrad)    dW[b] = X_b^T @ dY_b          (n = K, k = len, m = M): both operands MN-major, every segment split
+//                      into K chunks of `kchunk_steps` stages whose fp32 partials k_gt_finish adds (empty segment: zeros)
+__global__ void __launch_bounds__(1024) k_gt_build_segments(GProb* probs, int* total, const i64* __restrict__ ptr, const CUtensorMap* map_a,
                                     const CUtensorMap* map_b, unsigned char* out, const unsigned char* bias, int K, int M, int B,
-                                    int c_vec, i64 N, int* err) {
+                                    int c_vec, i64 N, int* err, int mode, int esize, int b_k, float* part, int kchunk_steps) {
   __shared__ int s_carry;
   __shared__ int s_w[32];
   if (threadIdx.x == 0) s_carry = 0;
-  {   // same validation of `ptr` as the other segment kernels (build_tile_prefix, matmul_tcgen05.cu)
+  {   // a ptr that is not a segment pointer over [0, N] leaves the launch without work and raises the flag
     int bad = 0;
     for (int b = threadIdx.x; b < B; b += blockDim.x) bad |= (ptr[b + 1] < ptr[b]) | (b == 0 && ptr[0] != 0) | (b == B - 1 && ptr[B] != N);
     if (__syncthreads_or(bad)) {
@@ -261,17 +283,28 @@ __global__ void k_gt_build_segments(GProb* probs, int* total, const i64* __restr
   }
   __syncthreads();
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int tiles_n = (M + GT_BN - 1) / GT_BN;
+  const int tiles_n = (M + GT_BN - 1) / GT_BN, bk = 128 / esize;
+  const int tiles_mn = ((K + GT_TM - 1) / GT_TM) * tiles_n;   // wgrad: output tiles of one dW[b]
   for (int base = 0; base < B; base += blockDim.x) {
     const int b = base + threadIdx.x;
     int tiles = 0;
     GProb p;
     if (b < B) {
       const i64 r0 = ptr[b], len = ptr[b + 1] - r0;
-      p.map_a = map_a; p.map_b = map_b; p.c = out + r0 * M * 2; p.bias = bias ? bias + (i64)b * M * 2 : nullptr;
-      p.ldc = M; p.n = (int)len; p.k = K; p.m = M; p.a_row0 = (int)r0; p.b_z = b; p.a_mn = 0; p.b_k = 0; p.c_vec = c_vec;
-      p.tiles_n = tiles_n; p.ksplit = 1; p.ksteps_chunk = (K + GT_BK - 1) / GT_BK; p.part = nullptr;
-      tiles = (int)((len + GT_TM - 1) / GT_TM) * tiles_n;
+      memset(&p, 0, sizeof(p));
+      p.map_a = map_a; p.map_b = map_b; p.ldc = M; p.m = M; p.a_off = (int)r0; p.tiles_n = tiles_n; p.c_vec = c_vec;
+      if (mode == 0) {
+        p.c = out + r0 * M * esize; p.bias = bias ? bias + (i64)b * M * esize : nullptr;
+        p.n = (int)len; p.k = K; p.b_z = b; p.b_k = b_k; p.c_f32 = esize == 4;
+        p.ksplit = 1; p.ksteps_chunk = (K + bk - 1) / bk;
+        tiles = (int)((len + GT_TM - 1) / GT_TM) * tiles_n;
+      } else {
+        p.c = out + (i64)b * K * M * esize;
+        p.n = K; p.k = (int)len; p.a_mn = 1; p.b_k0 = (int)r0; p.zero_ktail = 1;
+        p.ksteps_chunk = kchunk_steps;
+        p.ksplit = (int)((len + (i64)kchunk_steps * bk - 1) / ((i64)kchunk_steps * bk));
+        tiles = tiles_mn * p.ksplit;
+      }
     }
     int inc = tiles;
 #pragma unroll
@@ -284,7 +317,13 @@ __global__ void k_gt_build_segments(GProb* probs, int* total, const i64* __restr
     int pre = 0, tot = 0;
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { if (w < wid) pre += s_w[w]; tot += s_w[w]; }
     const int c0 = s_carry;
-    if (b < B) { p.tile0 = c0 + pre + inc - tiles; probs[b] = p; }
+    if (b < B) {
+      p.tile0 = c0 + pre + inc - tiles;
+      // wgrad: every segment has the same output tile grid, so tile0 / tiles_mn numbers the K chunks of all segments
+      // consecutively — chunk c of this segment owns partial buffer tile0 / tiles_mn + c
+      if (mode == 1) p.part = part + (i64)(p.tile0 / tiles_mn) * K * M;
+      probs[b] = p;
+    }
     __syncthreads();
     if (threadIdx.x == 0) s_carry = c0 + tot;
     __syncthreads();
@@ -297,7 +336,7 @@ template <bool BF16>
 __global__ void k_gt_finish(const GProb* __restrict__ probs, int P) {
   for (int b = blockIdx.y; b < P; b += gridDim.y) {
     const GProb pb = probs[b];
-    if (pb.ksplit <= 1) continue;
+    if (pb.part == nullptr) continue;
     const i64 nm = (i64)pb.n * pb.m;
     for (i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x; i < nm; i += (i64)gridDim.x * blockDim.x) {
       float v = 0.f;
@@ -306,6 +345,23 @@ __global__ void k_gt_finish(const GProb* __restrict__ probs, int P) {
       if (pb.bias) v += ld_bias<BF16>(pb.bias, col);
       reinterpret_cast<unsigned short*>(pb.c)[r * pb.ldc + col] = (unsigned short)(pack2<BF16>(v, 0.f) & 0xffffu);
     }
+  }
+}
+
+// W[b] [K, M] -> Wt[b] [M, K] (TF32 wgmma reads both operands K-major)
+__global__ void k_transpose_w_f32(const float* __restrict__ w, float* __restrict__ wt, int K, int M) {
+  __shared__ float tile[32][33];
+  const float* src = w + (size_t)blockIdx.z * K * M;
+  float* dst = wt + (size_t)blockIdx.z * K * M;
+  const int k0 = blockIdx.y * 32, m0 = blockIdx.x * 32;
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+    const int k = k0 + i, m = m0 + threadIdx.x;
+    tile[i][threadIdx.x] = (k < K && m < M) ? src[(size_t)k * M + m] : 0.f;
+  }
+  __syncthreads();
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+    const int m = m0 + i, k = k0 + threadIdx.x;
+    if (m < M && k < K) dst[(size_t)m * K + k] = tile[threadIdx.x][i];
   }
 }
 
@@ -323,14 +379,15 @@ EncodeTiledFn gt_encode() {
   return fn;
 }
 
-// 16-bit tensor, innermost dimension contiguous: dims / strides (bytes, for dims 1..) / box, 128-byte swizzle, zero fill
-int gt_map(CUtensorMap* m, const void* ptr, bool bf16, int rank, const cuuint64_t* dims, const cuuint64_t* strides, const cuuint32_t* box) {
+// innermost dimension contiguous: dims / strides (bytes, for dims 1..) / box, 128-byte swizzle, zero fill
+int gt_map(CUtensorMap* m, const void* ptr, int et, int rank, const cuuint64_t* dims, const cuuint64_t* strides, const cuuint32_t* box) {
   EncodeTiledFn enc = gt_encode();
   PYGB_CHECK(enc != nullptr, PYGB200_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
   cuuint32_t estr[3] = {1, 1, 1};
-  const CUresult r = enc(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank,
-                         const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const CUtensorMapDataType dt = et == ET_TF32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                 : et == ET_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const CUresult r = enc(m, dt, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled failed with code " + std::to_string((int)r));
     return PYGB200_ERR_CUDA;
@@ -338,27 +395,73 @@ int gt_map(CUtensorMap* m, const void* ptr, bool bf16, int rank, const cuuint64_
   return PYGB200_OK;
 }
 
-constexpr size_t GT_SMEM = 1024 + (size_t)GT_STAGES * GT_STAGE_BYTES + (2 * GT_STAGES + 4) * 8 + 16;
+constexpr size_t GT_SMEM = 1024 + (size_t)GT_STAGES * GT_STAGE_BYTES + 2 * (size_t)GT_OUT_BYTES + 2 * GT_STAGES * 8;
 
-int gt_launch(const GProb* probs, int P, const int* total, i64 tiles_bound, bool bf16, cudaStream_t st) {
-  int dev = 0, sms = 148;
+int num_sms() {
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int grid = (int)std::max<i64>(1, std::min<i64>(tiles_bound, sms));
+  return sms;
+}
+
+template <int ET, int LAYOUT>
+int gt_launch_et(const GProb* probs, int P, const int* total, int grid, cudaStream_t st) {
+  PYGB_CUDA(cudaFuncSetAttribute(k_grouped_wgmma<ET, LAYOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GT_SMEM));
+  k_grouped_wgmma<ET, LAYOUT><<<grid, GT_NT, GT_SMEM, st>>>(probs, P, total);
+  return PYGB200_OK;
+}
+
+template <int LAYOUT>
+int gt_launch_16(const GProb* probs, int P, const int* total, int grid, bool bf16, cudaStream_t st) {
+  return bf16 ? gt_launch_et<ET_BF16, LAYOUT>(probs, P, total, grid, st) : gt_launch_et<ET_F16, LAYOUT>(probs, P, total, grid, st);
+}
+
+int gt_launch(const GProb* probs, int P, const int* total, i64 tiles_bound, int et, int layout, const char* name, cudaStream_t st) {
+  const int grid = (int)std::max<i64>(1, std::min<i64>(tiles_bound, num_sms()));
   void* tk = prof_begin(st);
-  if (bf16) {
-    PYGB_CUDA(cudaFuncSetAttribute(k_grouped_tc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GT_SMEM));
-    k_grouped_tc<true><<<grid, GT_NT, GT_SMEM, st>>>(probs, P, total);
-  } else {
-    PYGB_CUDA(cudaFuncSetAttribute(k_grouped_tc<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GT_SMEM));
-    k_grouped_tc<false><<<grid, GT_NT, GT_SMEM, st>>>(probs, P, total);
-  }
-  prof_end(tk, "grouped_gemm", st, tiles_bound);
+  const bool bf16 = et == ET_BF16;
+  const int rc = et == ET_TF32 ? gt_launch_et<ET_TF32, LAY_FWD>(probs, P, total, grid, st)
+                 : layout == LAY_FWD ? gt_launch_16<LAY_FWD>(probs, P, total, grid, bf16, st)
+                 : layout == LAY_WGRAD ? gt_launch_16<LAY_WGRAD>(probs, P, total, grid, bf16, st)
+                                       : gt_launch_16<LAY_ANY>(probs, P, total, grid, bf16, st);
+  if (rc != PYGB200_OK) return rc;
+  prof_end(tk, name, st, tiles_bound);
+  PYGB_LAUNCH_CHECK();
+  return PYGB200_OK;
+}
+
+int finish_launch(const GProb* probs, int P, bool bf16, cudaStream_t st) {
+  const dim3 grid(64, (unsigned)std::min(P, 4096));
+  if (bf16) k_gt_finish<true><<<grid, 256, 0, st>>>(probs, P);
+  else k_gt_finish<false><<<grid, 256, 0, st>>>(probs, P);
   PYGB_LAUNCH_CHECK();
   return PYGB200_OK;
 }
 
 inline bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+// Segment-mode launch shared by the three segment paths: upload the two tensor maps, build the problem list from `ptr`
+// on the device, run the GEMM (and, for the weight gradient, the ordered sum of the K chunks).
+int segment_run(const CUtensorMap (&hm)[2], const i64* ptr_dev, void* out, const void* bias, i64 N, i64 K, i64 M, i64 B, int et,
+                int mode, int c_vec, int b_k, int kchunk_steps, size_t part_bytes, i64 tiles_bound, cudaStream_t st) {
+  const size_t prob_off = 256, total_off = prob_off + (((size_t)B * sizeof(GProb) + 15) & ~(size_t)15);
+  const size_t part_off = (total_off + 16 + 255) & ~(size_t)255;
+  AsyncScratch sc;   // (freed on every return path)
+  if (int e = sc.alloc(part_off + part_bytes, st)) return e;
+  unsigned char* dbuf = (unsigned char*)sc.p;
+  PYGB_CUDA(cudaMemcpyAsync(dbuf, hm, sizeof(hm), cudaMemcpyHostToDevice, st));
+  const CUtensorMap* dm = reinterpret_cast<const CUtensorMap*>(dbuf);
+  GProb* probs = reinterpret_cast<GProb*>(dbuf + prob_off);
+  int* total = reinterpret_cast<int*>(dbuf + total_off);
+  k_gt_build_segments<<<1, 1024, 0, st>>>(probs, total, ptr_dev, dm, dm + 1, reinterpret_cast<unsigned char*>(out),
+                                          reinterpret_cast<const unsigned char*>(bias), (int)K, (int)M, (int)B, c_vec, N,
+                                          mm_error_flag_dev(), mode, et == ET_TF32 ? 4 : 2, b_k,
+                                          reinterpret_cast<float*>(dbuf + part_off), kchunk_steps);
+  PYGB_LAUNCH_CHECK();
+  if (int e = gt_launch(probs, (int)B, total, tiles_bound, et, mode == 0 ? LAY_FWD : LAY_WGRAD, "segment_matmul", st)) return e;
+  if (mode == 1) return finish_launch(probs, (int)B, et == ET_BF16, st);
+  return PYGB200_OK;
+}
 
 }  // namespace
 
@@ -383,9 +486,8 @@ bool grouped_tc_supported(const pygb200_gemm_problem* ps, i64 count, int dtype) 
 
 int grouped_matmul_tc(const pygb200_gemm_problem* ps, i64 count, int dtype, cudaStream_t st) {
   const bool bf16 = dtype == PYGB200_BF16;
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int et = bf16 ? ET_BF16 : ET_F16;
+  const int sms = num_sms();
   // Split-K plan: a weight-gradient-shaped list (few output tiles, very long K: dW = X^T dY of a HeteroDictLinear) would
   // keep a handful of CTAs busy for thousands of K steps.  When the output tiles do not fill the machine twice, every
   // problem's K steps are cut into chunks (>= 8 steps = 512 of K each) that become work items of their own; chunk c
@@ -399,7 +501,7 @@ int grouped_matmul_tc(const pygb200_gemm_problem* ps, i64 count, int dtype, cuda
   for (i64 i = 0; i < count && want > 1; ++i) {
     const auto& q = ps[i];
     if (q.n <= 0 || q.m <= 0 || q.k <= 0) continue;
-    const i64 ksteps = (q.k + GT_BK - 1) / GT_BK;
+    const i64 ksteps = (q.k + 63) / 64;
     const i64 sp = std::max<i64>(1, std::min<i64>(want, ksteps / 8));
     const size_t bytes = (size_t)sp * q.n * q.m * 4;
     if (sp > 1 && part_bytes + bytes <= ((size_t)256 << 20)) { ksplit[(size_t)i] = (int)sp; part_bytes += (bytes + 255) & ~(size_t)255; }
@@ -430,14 +532,15 @@ int grouped_matmul_tc(const pygb200_gemm_problem* ps, i64 count, int dtype, cuda
     } else if (q.n > 0 && q.m > 0) {
       CUtensorMap ma, mb;
       cuuint64_t d[3], s[2]; cuuint32_t box[3];
-      if (!q.a_colmajor) { d[0] = (cuuint64_t)q.k; d[1] = (cuuint64_t)q.n; s[0] = (cuuint64_t)q.lda * 2; box[0] = 64; box[1] = GT_TM; }
-      else { d[0] = (cuuint64_t)q.n; d[1] = (cuuint64_t)q.k; s[0] = (cuuint64_t)q.lda * 2; box[0] = 64; box[1] = 64; }
-      rc = gt_map(&ma, q.a, bf16, 2, d, s, box);
+      if (!q.a_colmajor) { d[0] = (cuuint64_t)q.k; d[1] = (cuuint64_t)q.n; box[0] = 64; box[1] = GT_TM; }
+      else { d[0] = (cuuint64_t)q.n; d[1] = (cuuint64_t)q.k; box[0] = 64; box[1] = 64; }
+      s[0] = (cuuint64_t)q.lda * 2;
+      rc = gt_map(&ma, q.a, et, 2, d, s, box);
       if (rc != PYGB200_OK) break;
-      if (!q.b_colmajor) { d[0] = (cuuint64_t)q.m; d[1] = (cuuint64_t)q.k; }
-      else { d[0] = (cuuint64_t)q.k; d[1] = (cuuint64_t)q.m; }
-      d[2] = 1; s[0] = (cuuint64_t)q.ldb * 2; s[1] = s[0] * d[1]; box[0] = 64; box[1] = 64; box[2] = 1;
-      rc = gt_map(&mb, q.b, bf16, 3, d, s, box);
+      if (!q.b_colmajor) { d[0] = (cuuint64_t)q.m; d[1] = (cuuint64_t)q.k; box[1] = 64; }
+      else { d[0] = (cuuint64_t)q.k; d[1] = (cuuint64_t)q.m; box[1] = GT_BN; }
+      d[2] = 1; s[0] = (cuuint64_t)q.ldb * 2; s[1] = s[0] * d[1]; box[0] = 64; box[2] = 1;
+      rc = gt_map(&mb, q.b, et, 3, d, s, box);
       if (rc != PYGB200_OK) break;
       hmaps[2 * i] = ma; hmaps[2 * i + 1] = mb;
       p.map_a = dmaps + 2 * i; p.map_b = dmaps + 2 * i + 1;
@@ -445,7 +548,7 @@ int grouped_matmul_tc(const pygb200_gemm_problem* ps, i64 count, int dtype, cuda
       p.a_mn = q.a_colmajor ? 1 : 0; p.b_k = q.b_colmajor ? 1 : 0;
       p.c_vec = (al16(q.c) && q.ldc % 8 == 0) ? 1 : 0;
       p.tiles_n = (int)((q.m + GT_BN - 1) / GT_BN);
-      const int ksteps = (int)((q.k + GT_BK - 1) / GT_BK);
+      const int ksteps = (int)((q.k + 63) / 64);
       p.ksplit = ksplit[(size_t)i];
       p.ksteps_chunk = (ksteps + p.ksplit - 1) / p.ksplit;
       p.ksplit = (ksteps + p.ksteps_chunk - 1) / p.ksteps_chunk;   // (no empty chunk)
@@ -462,20 +565,15 @@ int grouped_matmul_tc(const pygb200_gemm_problem* ps, i64 count, int dtype, cuda
     *reinterpret_cast<int*>(h.data() + total_off) = (int)tiles;
     // pageable source: the copy is staged by the driver before the call returns, so `h` may die at the end of the scope
     if (cudaMemcpyAsync(dbuf, h.data(), h.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) rc = PYGB200_ERR_CUDA;
-    if (rc == PYGB200_OK) rc = gt_launch(reinterpret_cast<const GProb*>(dbuf + prob_off), (int)count, reinterpret_cast<const int*>(dbuf + total_off), tiles, bf16, st);
-    if (rc == PYGB200_OK && any_split) {
-      const dim3 grid(64, (unsigned)std::min<i64>(count, 4096));
-      if (bf16) k_gt_finish<true><<<grid, 256, 0, st>>>(reinterpret_cast<const GProb*>(dbuf + prob_off), (int)count);
-      else k_gt_finish<false><<<grid, 256, 0, st>>>(reinterpret_cast<const GProb*>(dbuf + prob_off), (int)count);
-      count_launch();
-      if (cudaGetLastError() != cudaSuccess) rc = PYGB200_ERR_CUDA;
-    }
+    const GProb* dprobs = reinterpret_cast<const GProb*>(dbuf + prob_off);
+    if (rc == PYGB200_OK) rc = gt_launch(dprobs, (int)count, reinterpret_cast<const int*>(dbuf + total_off), tiles, et, LAY_ANY, "grouped_gemm", st);
+    if (rc == PYGB200_OK && any_split) rc = finish_launch(dprobs, (int)count, bf16, st);
   }
   return rc;
 }
 
-// ---- pyg::segment_matmul for the shapes the specialised kernel does not take
-bool segment_tc_general_supported(i64 N, i64 K, i64 M, i64 B, int dtype, const void* x, const void* w, const void* out) {
+// ---- pyg::segment_matmul, bf16 / fp16
+bool segment_tc_supported(i64 N, i64 K, i64 M, i64 B, int dtype, const void* x, const void* w, const void* out) {
   if (dtype != PYGB200_BF16 && dtype != PYGB200_F16) return false;
   static const bool off = getenv("PYGB200_NO_GROUPED_TC") != nullptr;
   if (off) return false;
@@ -485,36 +583,77 @@ bool segment_tc_general_supported(i64 N, i64 K, i64 M, i64 B, int dtype, const v
   return al16(x) && al16(w) && al16(out);
 }
 
-int segment_matmul_tc_general(const void* x, const i64* ptr_dev, const void* w, const void* bias, void* out, i64 N, i64 K, i64 M,
-                              i64 B, int dtype, cudaStream_t st) {
-  const bool bf16 = dtype == PYGB200_BF16;
+int segment_matmul_tc(const void* x, const i64* ptr_dev, const void* w, const void* bias, void* out, i64 N, i64 K, i64 M, i64 B,
+                      int dtype, cudaStream_t st) {
+  const int et = dtype == PYGB200_BF16 ? ET_BF16 : ET_F16;
   CUtensorMap hm[2];
-  {
-    cuuint64_t d[3] = {(cuuint64_t)K, (cuuint64_t)N, 1}, s[2] = {(cuuint64_t)K * 2, 0};
-    cuuint32_t box[3] = {64, GT_TM, 1};
-    if (int e = gt_map(&hm[0], x, bf16, 2, d, s, box)) return e;
-    cuuint64_t dw[3] = {(cuuint64_t)M, (cuuint64_t)K, (cuuint64_t)B}, sw[2] = {(cuuint64_t)M * 2, (cuuint64_t)K * M * 2};
-    cuuint32_t bw[3] = {64, 64, 1};
-    if (int e = gt_map(&hm[1], w, bf16, 3, dw, sw, bw)) return e;
-  }
-  const size_t prob_off = 256, total_off = prob_off + (((size_t)B * sizeof(GProb) + 15) & ~(size_t)15);
-  AsyncScratch sc;
-  if (int e = sc.alloc(total_off + 16, st)) return e;
-  unsigned char* dbuf = (unsigned char*)sc.p;
-  int rc = PYGB200_OK;
-  if (cudaMemcpyAsync(dbuf, hm, sizeof(hm), cudaMemcpyHostToDevice, st) != cudaSuccess) rc = PYGB200_ERR_CUDA;
-  if (rc == PYGB200_OK) {
-    const CUtensorMap* dm = reinterpret_cast<const CUtensorMap*>(dbuf);
-    k_gt_build_segments<<<1, 1024, 0, st>>>(reinterpret_cast<GProb*>(dbuf + prob_off), reinterpret_cast<int*>(dbuf + total_off), ptr_dev, dm,
-                                            dm + 1, reinterpret_cast<unsigned char*>(out), reinterpret_cast<const unsigned char*>(bias),
-                                            (int)K, (int)M, (int)B, 1 /* rows of out are M * 2 bytes apart, M % 8 == 0 */, N, mm_error_flag_dev());
-    count_launch();
-    if (cudaGetLastError() != cudaSuccess) rc = PYGB200_ERR_CUDA;
-  }
-  if (rc == PYGB200_OK)
-    rc = gt_launch(reinterpret_cast<const GProb*>(dbuf + prob_off), (int)B, reinterpret_cast<const int*>(dbuf + total_off),
-                   (N / GT_TM + B) * ((M + GT_BN - 1) / GT_BN), bf16, st);
-  return rc;
+  cuuint64_t d[3] = {(cuuint64_t)K, (cuuint64_t)N, 1}, s[2] = {(cuuint64_t)K * 2, 0};
+  cuuint32_t box[3] = {64, GT_TM, 1};
+  if (int e = gt_map(&hm[0], x, et, 2, d, s, box)) return e;
+  cuuint64_t dw[3] = {(cuuint64_t)M, (cuuint64_t)K, (cuuint64_t)B}, sw[2] = {(cuuint64_t)M * 2, (cuuint64_t)K * M * 2};
+  cuuint32_t bw[3] = {64, 64, 1};
+  if (int e = gt_map(&hm[1], w, et, 3, dw, sw, bw)) return e;
+  // rows of out are M * 2 bytes apart and M % 8 == 0: 16-byte aligned
+  return segment_run(hm, ptr_dev, out, bias, N, K, M, B, et, 0, 1, 0, 0, 0, (N / GT_TM + B) * ((M + GT_BN - 1) / GT_BN), st);
+}
+
+// ---- pyg::segment_matmul, fp32 storage with TF32 math (taken when the caller allows TF32:
+// torch.get_float32_matmul_precision() != 'highest', like the reference's TensorOp kernel, matmul_kernel.cu:159-190).
+// TF32 wgmma reads both operands K-major, so W is transposed once per call into a [B, M, K] scratch.
+bool tf32_supported(i64 N, i64 K, i64 M, i64 B, const void* x, const void* w, const void* out) {
+  if (K < 64 || K > 256 || K % 64 != 0) return false;
+  if (M < 32 || M > 256 || M % 32 != 0) return false;
+  if (B < 1 || B > MAX_SEG || N < 1 || N >= ((i64)1 << 31) || B * K >= ((i64)1 << 31)) return false;
+  return al16(x) && al16(w) && al16(out);
+}
+
+int segment_matmul_tf32(const void* x, const i64* ptr_dev, const void* w, const void* bias, void* out, i64 N, i64 K, i64 M, i64 B,
+                        cudaStream_t st) {
+  AsyncScratch sc;   // (freed on every return path)
+  if (int e = sc.alloc((size_t)B * K * M * 4, st)) return e;
+  float* wt = (float*)sc.p;
+  k_transpose_w_f32<<<dim3((unsigned)((M + 31) / 32), (unsigned)((K + 31) / 32), (unsigned)B), dim3(32, 8), 0, st>>>(
+      (const float*)w, wt, (int)K, (int)M);
+  PYGB_LAUNCH_CHECK();
+  CUtensorMap hm[2];
+  cuuint64_t d[3] = {(cuuint64_t)K, (cuuint64_t)N, 1}, s[2] = {(cuuint64_t)K * 4, 0};
+  cuuint32_t box[3] = {32, GT_TM, 1};
+  if (int e = gt_map(&hm[0], x, ET_TF32, 2, d, s, box)) return e;
+  cuuint64_t dw[3] = {(cuuint64_t)K, (cuuint64_t)M, (cuuint64_t)B}, sw[2] = {(cuuint64_t)K * 4, (cuuint64_t)K * M * 4};
+  cuuint32_t bw[3] = {32, GT_BN, 1};
+  if (int e = gt_map(&hm[1], wt, ET_TF32, 3, dw, sw, bw)) return e;
+  return segment_run(hm, ptr_dev, out, bias, N, K, M, B, ET_TF32, 0, 1, 1, 0, 0, (N / GT_TM + B) * ((M + GT_BN - 1) / GT_BN), st);
+}
+
+// ---- weight gradient dW[b] = X_b^T @ dY_b, bf16 / fp16 (replaces the B torch::matmul calls + at::stack of
+// SegmentMatmul::backward, pyg_lib/csrc/ops/autograd/matmul_kernel.cpp:92-107; deterministic like them)
+bool wgrad_tc_supported(i64 N, i64 K, i64 M, i64 B, int dtype, const void* x, const void* dy, const void* dw) {
+  if (dtype != PYGB200_BF16 && dtype != PYGB200_F16) return false;
+  if (K != 128) return false;
+  if (M < 64 || M > 256 || M % 64 != 0) return false;
+  if (B < 1 || B > MAX_SEG || N < 1 || N >= ((i64)1 << 31)) return false;
+  return al16(x) && al16(dy) && al16(dw);
+}
+
+int segment_wgrad_tc(const void* x, const i64* ptr_dev, const void* dy, void* dw, i64 N, i64 K, i64 M, i64 B, int dtype,
+                     cudaStream_t st) {
+  const int et = dtype == PYGB200_BF16 ? ET_BF16 : ET_F16;
+  CUtensorMap hm[2];
+  cuuint64_t d[3] = {(cuuint64_t)K, (cuuint64_t)N, 1}, s[2] = {(cuuint64_t)K * 2, 0};
+  cuuint32_t box[3] = {64, 64, 1};   // MN-major A = X^T: box [64 columns of X x 64 rows]
+  if (int e = gt_map(&hm[0], x, et, 2, d, s, box)) return e;
+  cuuint64_t dd[3] = {(cuuint64_t)M, (cuuint64_t)N, 1}, sd[2] = {(cuuint64_t)M * 2, (cuuint64_t)N * M * 2};
+  if (int e = gt_map(&hm[1], dy, et, 3, dd, sd, box)) return e;
+  // K chunks of 2048 rows (32 stages) at least; longer when the partials of (N / chunk + B) chunks would pass 256 MB
+  const i64 km_bytes = K * M * 4, slots = ((i64)256 << 20) / km_bytes;
+  i64 chunk = 2048;
+  if (slots > B + 1) chunk = std::max<i64>(chunk, ceil_div(N, slots - B - 1));
+  else chunk = std::max<i64>(N, 64);
+  chunk = ceil_div(chunk, (i64)64) * 64;
+  const i64 chunks = ceil_div(N, chunk) + B;
+  const i64 tiles_mn = ceil_div(K, (i64)GT_TM) * ceil_div(M, (i64)GT_BN);
+  return segment_run(hm, ptr_dev, dw, nullptr, N, K, M, B, et, 1, 1, 0, (int)(chunk / 64), (size_t)chunks * km_bytes,
+                     chunks * tiles_mn, st);
 }
 
 }  // namespace pygb200

@@ -7,7 +7,7 @@
 //     w = (random64() % (2^64-1)) + INT64_MIN, reads block elements from index 127 down to 0 and
 //     slices each word into 16/32/64-bit fields from the low end.
 //
-// B200 design: the mt19937 *raw* (untempered) state stream is materialised in HBM by one CTA using
+// Design: the mt19937 *raw* (untempered) state stream is materialised in HBM by one CTA using
 // the linear recurrence  raw[m] = raw[m-227] ^ T(raw[m-624], raw[m-623])  unrolled KL times, so that
 // up to min(227*KL, 623) words are produced per barrier instead of one 624-word twist per three
 // barriers.  Tempering, 64-bit assembly and the randint transform happen at the point of use.
@@ -196,8 +196,7 @@ __global__ void __launch_bounds__(640) k_mt_jump_prestep(u32* __restrict__ raw, 
 // pre-step).  The last CTA to finish publishes the new length.
 // The jump itself is ~10 k XORs of history words per thread: the history the polynomial reads (MT_JUMP_HIST words,
 // 85 KB) is staged in shared memory first — read from L2 inside the bit loop, every XOR waited for one L2 round trip
-// (a while(bits) loop is not unrolled, so the loads did not overlap) and a 131 072-word chunk took 2.0 ms, of which the
-// generation proper is ~25 us (ncu launch list, profiles/launches_big_r2.csv).
+// (a while(bits) loop is not unrolled, so the loads did not overlap) and the jump, not the generation, dominated a chunk.
 constexpr int MT_JUMP_HIST = 19938 + MT_N + 62;   // highest history index read: deg(g) <= 19937, + 623; rounded to 20 624
 template <int KL>
 __global__ void __launch_bounds__(640) k_mt_jump_generate(u32* __restrict__ raw, i64* generated, const i64* jump_base,

@@ -1,4 +1,4 @@
-// pyg_lib_b200/csrc/sampler.cu — neighbor_sample / hetero_neighbor_sample for sm_100a.
+// pyg_lib_b200/csrc/sampler.cu — neighbor_sample / hetero_neighbor_sample for sm_90a (H100).
 //
 // Replaces the single-threaded CPU loops of pyg_lib/csrc/sampler/cpu/neighbor_kernel.cpp
 // (NeighborSampler :22-328, homogeneous sample<> :337-514, hetero sample<> :529-841) and reproduces
@@ -1540,7 +1540,7 @@ using namespace pygb200;
 // ------------------------------------------------------------------------------------- handle
 struct pygb200_sampler {
   int device = -1;
-  int sm_count = 148;
+  int sm_count = 132;
   struct TypeBuf {
     DevBuf nodes, batch, slot, keys, vals;
     // v2: packed tables (node id << 32 | value) and the slot lists that say which entries a run touched, TWO of each:

@@ -2,9 +2,9 @@
 // anonymous namespace (it uses PassArgs, NodeRec, sample_draws, pdl_enter, last_block, ... from there).
 //
 // Same results as the other schedules (bit-exact vs neighbor_kernel.cpp:337-514 / 529-841), different data path, built
-// from what tools/p2p_microbench.cu measured on B200: random 8-byte atomics on a table larger than L2 run at ~30 G/s
-// when an insert is ONE atomic and at ~12 G/s when it is CAS(keys) + min(vals) on two arrays; random 8-byte loads
-// at ~65 G/s; a peer GPU takes ~9 G CAS/s and ~700 GB/s of coalesced stores over NVLink.  So:
+// from what tools/p2p_microbench.cu measures: random 8-byte atomics on a table larger than L2 run more than twice as fast
+// when an insert is ONE atomic than when it is CAS(keys) + min(vals) on two arrays; random 8-byte loads are faster still;
+// a peer GPU takes CAS and coalesced stores over NVLink at a fraction of local rates.  So:
 //   * packed table: one u64 slot = (node id : 32 | value : 32); value = V2_POS | flat position of the running pass
 //     until ids are assigned, else the node's local id.  Insert = one CAS (+ one min only when the key was already
 //     there with a larger position).  Needs node ids < 2^32 - 1, pass positions and local ids < 2^31 (checked by
@@ -447,8 +447,7 @@ __global__ void __launch_bounds__(NT) k_v2_mark(const PassArgs a) {
 // inserts into this table (then nobody will read it).
 // Four edges per thread: the kernel is a chain of dependent loads per edge (ref -> rank of the ref's position ->
 // store), and with one edge per thread in flight — the loads of an unrolled iteration could not move above the stores
-// of the previous one — it ran at 3.5 % issue utilisation: 357 us for 6 M edges (profiles/ncu_summary_r2.json, first
-// capture).  Now the four refs and their four rank lookups are issued together through the read-only path (nothing
+// of the previous one — it ran at a few percent issue utilisation in a profile of the first version.  Now the four refs and their four rank lookups are issued together through the read-only path (nothing
 // this kernel writes is read by it, except colv by the same thread).
 __device__ __forceinline__ i64 v2_rank_of(const PassArgs& a, u32 q) {
   return __ldg(&a.mtile[q / ETILE]) + (i64)__ldg(&a.erank[q]);

@@ -1,4 +1,4 @@
-// pyg_lib_b200/csrc/subgraph.cu — induced subgraph (pyg::subgraph) for sm_100a.
+// pyg_lib_b200/csrc/subgraph.cu — induced subgraph (pyg::subgraph) for sm_90a (H100).
 //
 // Replaces subgraph_kernel (pyg_lib/csrc/sampler/cpu/subgraph_kernel.cpp:13-89), same two sweeps with the
 // prefix sum between them, each node row handled by one warp:
@@ -257,7 +257,7 @@ __global__ void __launch_bounds__(NT) k_seg_gather(const i64* __restrict__ offs,
 using namespace pygb200;
 
 struct pygb200_subgraph {
-  int device = 0, sm_count = 148;
+  int device = 0, sm_count = 132;
   DevBuf keys, vals, slot, flag, ids, deg, offs, tiles, misc, segs;   // misc: {total, err}; segs: hetero relabel segment lists
   u64 tcap = 0;
   i64 n = 0;            // node count of the pending count() (fill() must follow with the same inputs)

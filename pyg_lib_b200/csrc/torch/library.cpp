@@ -19,7 +19,7 @@ TORCH_LIBRARY_FRAGMENT(pyg, m) {
 // tensors raises one clear message that says what to do.
 static void cpu_not_supported(const c10::OperatorHandle& op, c10::DispatchKeySet, torch::jit::Stack*) {
   TORCH_CHECK(false, "pyg_lib_b200: '", op.schema().name(), "' was called with CPU tensors. This build implements the CUDA "
-              "(sm_100a) path only and has no CPU fallback: move the graph / feature tensors to a CUDA device, or use the "
+              "(sm_90a) path only and has no CPU fallback: move the graph / feature tensors to a CUDA device, or use the "
               "stock pyg-lib package for CPU sampling (set PYG_LIB_B200_NO_ALIAS=1 to keep `import pyg_lib` from "
               "resolving to this package).");
 }

@@ -169,7 +169,7 @@ at::Tensor segment_matmul_autograd(const at::Tensor& input, const at::Tensor& pt
 TORCH_LIBRARY_FRAGMENT(pyg, m) {
   m.def(TORCH_SELECTIVE_SCHEMA("pyg::grouped_matmul(Tensor[] input, Tensor[] other) -> Tensor[]"));
   m.def(TORCH_SELECTIVE_SCHEMA("pyg::segment_matmul(Tensor input, Tensor ptr, Tensor other) -> Tensor"));
-  // B200-only additions (not in the reference): fused bias epilogue and the weight-gradient kernel
+  // Additions of this package (not in the reference): fused bias epilogue and the weight-gradient kernel
   m.def(TORCH_SELECTIVE_SCHEMA("pyg::segment_matmul_bias(Tensor input, Tensor ptr, Tensor other, Tensor bias) -> Tensor"));
   m.def(TORCH_SELECTIVE_SCHEMA("pyg::segment_matmul_wgrad(Tensor input, Tensor ptr, Tensor grad_out) -> Tensor"));
 }

@@ -1,5 +1,5 @@
 """`pyg_lib.ops.segment_matmul` / `grouped_matmul` — same signatures, argument meaning and autograd
-behaviour as the reference (pyg_lib/ops/__init__.py:59-172), bound to the sm_100a kernels."""
+behaviour as the reference (pyg_lib/ops/__init__.py:59-172), bound to the sm_90a kernels."""
 from typing import List, Optional, Tuple
 
 import torch
@@ -15,7 +15,7 @@ def _flatten_apply(fn_cls, tensors: Tuple[Tensor, ...]):
 
 class GroupedMatmul(torch.autograd.Function):
     r"""Reference: pyg_lib/ops/__init__.py:59-96 (forward = one grouped launch; backward = two more
-    grouped launches on transposed *views*, which the B200 kernel reads through strides)."""
+    grouped launches on transposed *views*, which the CUDA kernels read through strides)."""
     @staticmethod
     def forward(ctx, *args: Tensor):
         ctx.save_for_backward(*args)

@@ -60,13 +60,20 @@ def main():
         for k, v in r[5].items(): out[f'hetero/{name}/eph/{k}'] = np_(v)
         out[f'hetero/{name}/rng_after'] = torch.get_rng_state().numpy()[:24 + 624 * 8].copy()
         print('hetero', name, sum(v.numel() for v in r[0].values()), 'edges')
+    lowp = {}   # bf16 / fp16 results in their own 16-bit encoding (lossless, half the bytes; tests/conftest.py decodes)
     for name, case in MATMUL_CASES.items():
         x, ptr, w = build_matmul(case)
         o = torch.ops.pyg.segment_matmul(x, ptr, w)
-        out[f'matmul/{name}/out'] = o.float().numpy()
+        if o.dtype == torch.bfloat16:
+            lowp[f'matmul/{name}/out'] = o.view(torch.int16).numpy().view(np.uint16)
+        elif o.dtype == torch.float16:
+            lowp[f'matmul/{name}/out'] = o.numpy()
+        else:
+            out[f'matmul/{name}/out'] = o.float().numpy()
         print('matmul', name, tuple(o.shape))
-    np.savez_compressed(osp.join(HERE, 'reference_outputs.npz'), **out)
-    print('wrote', osp.join(HERE, 'reference_outputs.npz'), os.path.getsize(osp.join(HERE, 'reference_outputs.npz')), 'bytes')
+    for fn, data in (('reference_outputs.npz', out), ('reference_outputs_lowp.npz', lowp)):
+        np.savez_compressed(osp.join(HERE, fn), **data)
+        print('wrote', osp.join(HERE, fn), os.path.getsize(osp.join(HERE, fn)), 'bytes')
 
 
 if __name__ == '__main__':

@@ -1,6 +1,11 @@
 """Run the reference (oracle/ref_parity.py, a subprocess: oracle/_ref/libpyg_ref.so and libpyg.so both register the
 pyg:: schemas) on inputs that may be too large to pickle: big tensors go through raw files under /dev/shm (or the
-temp dir) that the child maps with torch.from_file.  Used by tests/test_config_parity.py and bench.py's parity gate."""
+temp dir) that the child maps with torch.from_file.  Used by tests/golden/make_golden_config.py, which stores what
+the reference answered (tests/golden/config_parity.json: SHA-256 digests of every index tensor and of the generator
+state, hop counts; tests/golden/config_matmul_rows.npz: a fixed sample of matmul rows) for tests/test_config_parity.py,
+tests/test_refproc.py and bench.py's parity gate."""
+import hashlib
+import json
 import os
 import os.path as osp
 import shutil
@@ -106,3 +111,55 @@ def lowp_ulp_excess(out: torch.Tensor, ref: torch.Tensor, abs_tol=None) -> float
             d = (d - abs_tol[i:i + step].to(d.device)).clamp_min(0)
         worst = max(worst, float((d / (rel * rc.abs().clamp_min(1e-30))).max()))
     return worst
+
+
+# ------------------------------------------------------------------------------------ stored reference answers
+GOLDEN_JSON = osp.join(ROOT, 'tests', 'golden', 'config_parity.json')
+GOLDEN_ROWS = osp.join(ROOT, 'tests', 'golden', 'config_matmul_rows.npz')
+
+
+def digest(t) -> str:
+    """SHA-256 of a tensor's dtype, shape and bytes (None -> 'none'): bit-exact comparison without storing the tensor."""
+    if t is None:
+        return 'none'
+    a = t.detach().cpu().contiguous()
+    h = hashlib.sha256(f'{a.dtype}{tuple(a.shape)}'.encode())
+    h.update(a.view(torch.uint8).numpy().tobytes() if a.numel() else b'')
+    return h.hexdigest()
+
+
+def digest_homo(out) -> dict:
+    """One neighbor_sample result (row, col, node, eid, nph, eph) -> what the golden file stores of it."""
+    return dict(row=digest(out[0]), col=digest(out[1]), node=digest(out[2]), eid=digest(out[3]),
+                nph=[int(v) for v in out[4]], eph=[int(v) for v in out[5]], edges=int(out[0].numel()))
+
+
+def digest_hetero(out, rel=lambda k: k) -> dict:
+    """One hetero_neighbor_sample result; edge-type keys through `rel` (tuple -> 'src__rel__dst')."""
+    key = lambda k: rel(k) if isinstance(k, tuple) else k   # noqa: E731
+    res = {}
+    for i, name in enumerate(('row', 'col', 'node', 'eid')):
+        res[name] = None if out[i] is None else {key(k): digest(v) for k, v in sorted(out[i].items(), key=lambda kv: key(kv[0]))}
+    res['nph'] = {key(k): [int(x) for x in v] for k, v in out[4].items()}
+    res['eph'] = {key(k): [int(x) for x in v] for k, v in out[5].items()}
+    res['edges'] = int(sum(v.numel() for v in out[0].values()))
+    return res
+
+
+def golden(name: str) -> dict:
+    with open(GOLDEN_JSON) as f:
+        return json.load(f)[name]
+
+
+def golden_rows(name: str):
+    """(row indices, the reference's bf16 output at those rows) of a stored matmul case."""
+    import numpy as np
+    z = np.load(GOLDEN_ROWS)
+    return torch.from_numpy(z[name + '/rows'].astype(np.int64)), torch.from_numpy(z[name + '/y'].astype(np.int16)).view(torch.bfloat16)
+
+
+def compare_homo_golden(out, gold_call) -> dict:
+    """compare_homo against a stored (digested) reference call."""
+    d = digest_homo(out)
+    bad = [k for k in ('row', 'col', 'node', 'eid', 'nph', 'eph') if d[k] != gold_call[k]]
+    return {'bit_exact': not bad, 'mismatch': bad, 'edges': d['edges'], 'nodes': int(out[2].shape[0])}

@@ -1,4 +1,4 @@
-"""GPU parity: segment_matmul / grouped_matmul (torch.ops.pyg.* -> C ABI -> sm_100a kernels) vs the CPU
+"""GPU parity: segment_matmul / grouped_matmul (torch.ops.pyg.* -> C ABI -> sm_90a kernels) vs the CPU
 oracle, the reference-generated fixtures and a plain fp32 torch matmul.
 
 Tolerances (SURVEY 8c): fp32 'highest' atol 1e-5 (reference test: 1e-6 on 8x16 inputs,
@@ -128,8 +128,8 @@ def test_segment_matmul_errors(lib):
 @pytest.mark.parametrize('K,M', [(128, 128), (64, 64), (64, 128), (128, 64), (192, 64)])
 @pytest.mark.parametrize('with_bias', [False, True])
 def test_tcgen05_path(lib, dtype, K, M, with_bias):
-    """Shapes that take the tcgen05/TMA kernel (K, M multiples of 64): ragged segments incl. empty and
-    1-row ones, tiles that end mid-segment, more tiles than SMs."""
+    """K, M multiples of 64 on the wgmma/TMA kernel: ragged segments incl. empty and 1-row ones, tiles that end
+    mid-segment, more tiles than SMs."""
     g = torch.Generator().manual_seed(K * 1000 + M)
     lens = [0, 1, 127, 128, 129, 300, 0, 1000, 5, 4096, 77, 20000]
     ptr = torch.tensor([0] + lens).cumsum(0)
@@ -229,8 +229,8 @@ def _launch_delta(lib, fn):
 @pytest.mark.parametrize('K,M', [(32, 32), (96, 96), (512, 512), (1024, 64), (40, 24), (328, 520), (256, 1000), (8, 8)])
 def test_segment_matmul_general_tc_shapes(lib, dtype, K, M):
     """K / M outside {64,128,192,256} (VERDICT r1 missing #3: hidden sizes 32, 96, 512, 1024, and anything that is a
-    multiple of 8) run the general tcgen05 kernel of matmul_grouped_tc.cu — K loop over 64-wide stages, column tiles
-    of 256, TMA zero-fill for every tail — and must match a per-segment fp32 matmul like the specialised kernel."""
+    multiple of 8) run the wgmma kernel of matmul_grouped_tc.cu — K loop over 64-wide stages, column tiles
+    of 128, TMA zero-fill for every tail — and must match a per-segment fp32 matmul like the multiple-of-64 shapes."""
     g = torch.Generator().manual_seed(K * 1000 + M)
     lens = [0, 1, 127, 128, 129, 300, 0, 1000, 5, 2048, 77]
     ptr = torch.tensor([0] + lens).cumsum(0)

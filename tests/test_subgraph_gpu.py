@@ -1,4 +1,4 @@
-"""GPU parity: pyg::subgraph (torch op -> C ABI -> sm_100a kernels) vs the reference fixtures
+"""GPU parity: pyg::subgraph (torch op -> C ABI -> sm_90a kernels) vs the reference fixtures
 (tests/golden/subgraph_outputs.npz) and the CPU oracle.  Bit-exact."""
 import ctypes as C
 import os.path as osp

@@ -1,13 +1,12 @@
-"""Summarise `ncu --set full` reports into profiles/ncu_summary_r<N>.json (the file bench.py reads its per-launch
-DRAM traffic from).  Usage, in the container (reports come back from the GPU box in gpurun_out/):
+"""Summarise `ncu --set full` reports into one JSON file (per-kernel duration, DRAM traffic, ...).  Usage:
 
-    python tools/ncu_summary.py [--out profiles/ncu_summary_r2.json] sampler=gpurun_out/prof.ncu-rep [matmul=...]
+    python tools/ncu_summary.py [--out ncu_summary.json] sampler=prof.ncu-rep [matmul=...]
 
 Groups that are not given keep what the JSON already holds."""
 import csv, io, json, os, subprocess, sys
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), '..')
-OUT = os.path.join(ROOT, 'profiles', 'ncu_summary_r2.json')
+OUT = 'ncu_summary.json'
 KEEP = ['gpu__time_duration.sum', 'dram__bytes_read.sum', 'dram__bytes_write.sum',
         'gpu__dram_throughput.avg.pct_of_peak_sustained_elapsed',
         'sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active',

@@ -1,7 +1,7 @@
 // tools/p2p_microbench.cu — what NVLink peer memory gives a sampling kernel (design input for the frontier-sharded
 // sampler, DESIGN.md §6): rate of random 8-byte loads / stores / atomicCAS / red.min on LOCAL vs PEER memory,
 // coalesced peer store / load bandwidth, and the one-way latency of a flag between two GPUs.
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o /tmp/p2p tools/p2p_microbench.cu && /tmp/p2p
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o /tmp/p2p tools/p2p_microbench.cu && /tmp/p2p
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -53,6 +53,7 @@ int main() {
   CK(cudaSetDevice(0)); CK(cudaMalloc(&loc, slots * 8)); CK(cudaMalloc(&loc2, slots * 8)); CK(cudaMalloc(&sink, 8));
   CK(cudaSetDevice(peer)); CK(cudaMalloc(&rem, slots * 8)); CK(cudaMalloc(&rem2, slots * 8));
   CK(cudaSetDevice(0));
+  int sms = 0; CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
   cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
   const long n = 1 << 24;
   const char* names[] = {"load8", "store8", "CAS", "red.min", "CAS+red.min"};
@@ -62,7 +63,7 @@ int main() {
       CK(cudaMemset(loc, 0xff, slots * 8)); CK(cudaMemset(loc2, 0xff, slots * 8));
       CK(cudaSetDevice(peer)); CK(cudaMemset(rem, 0xff, slots * 8)); CK(cudaMemset(rem2, 0xff, slots * 8)); CK(cudaDeviceSynchronize());
       CK(cudaSetDevice(0));
-      for (int grid : {148 * 2, 148 * 8}) {
+      for (int grid : {sms * 2, sms * 8}) {
         k_random<<<grid, 256>>>(t, t2, slots - 1, n / 8, mode, sink);  // warm
         CK(cudaEventRecord(e0));
         k_random<<<grid, 256>>>(t, t2, slots - 1, n, mode, sink);
@@ -76,7 +77,7 @@ int main() {
   const long n16 = (long)slots / 2;  // 256 MB
   for (int dir = 0; dir < 3; ++dir) {
     const uint4* s = (const uint4*)(dir == 1 ? rem : loc); uint4* d = (uint4*)(dir == 0 ? rem2 : loc2);
-    for (int grid : {148, 148 * 4, 148 * 16}) {
+    for (int grid : {sms, sms * 4, sms * 16}) {
       k_copy16<<<grid, 256>>>(s, d, n16 / 8);
       CK(cudaEventRecord(e0));
       k_copy16<<<grid, 256>>>(s, d, n16);

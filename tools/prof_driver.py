@@ -1,11 +1,11 @@
-"""One steady-state invocation of every hot kernel family between cudaProfilerStart/Stop, for ncu (B200_PROFILING.md):
+"""One steady-state invocation of every hot kernel family between cudaProfilerStart/Stop, for a profiler such as ncu:
 
   ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches.csv python tools/prof_driver.py
   ncu --profile-from-start off --set full --clock-control none --import-source on -o gpurun_out/prof python tools/prof_driver.py
 
 Region: neighbor_sample 1024 seeds (latency schedule) and 65,536 seeds (throughput schedule) on the products-shaped graph, biased
-sampling with and without replacement, segment_matmul C3 (specialised tcgen05 kernel), grouped_matmul 8 x [100k,256]@[256,256]
-(general tcgen05 kernel, forward and the dW view)."""
+sampling with and without replacement, segment_matmul C3 and grouped_matmul 8 x [100k,256]@[256,256]
+(the wgmma kernel, forward and the dW view)."""
 import os
 import sys
 
