@@ -23,7 +23,6 @@
 
 #include <algorithm>
 #include <atomic>
-#include <chrono>
 #include <mutex>
 #include <vector>
 
@@ -162,7 +161,7 @@ struct PassArgs {
   int v2_writeback, o_shard;
   i64 x_off_bar, x_off_dst, x_off_eid, x_off_fref;               // byte offsets inside an exchange region
   i64 x_off_exc, x_off_exc_n, x_off_xcnt, x_exc_cap;             // ref exceptions: W lists of (position, ref), their lengths, my counter
-  u64 x_sig_epoch, x_wait_epoch, x_timeout_ns;                   // cross-GPU flags raised at the end / awaited at the start of a kernel (0 = none)
+  u64 x_sig_epoch, x_timeout_ns;                                 // cross-GPU flags raised at the end of a kernel (0 = none)
   int sd_begin, sd_end, sd_nph;                                  // seed pass: frontier-slice words its mark kernel sets (k_seed_end folded in; 0 = not)
   unsigned char* xpeer[16];        // exchange region of every rank (own one included), peer-mapped
 };
@@ -626,10 +625,7 @@ __device__ __forceinline__ void sample_draws(const PassArgs& a, const NodeRec& r
   }
 }
 
-__device__ __forceinline__ u32 v2_insert(u64* __restrict__ pk, int bits, u32 key, u32 p);   // (sampler_v2.cuh: packed table)
-
-// PK: the dst type's table is the packed one (slot = node id : 32 | value : 32; sampler_v2.cuh) — one CAS per insert
-template <typename idx_t, bool PHASED, bool PK = false>
+template <typename idx_t, bool PHASED>
 __device__ __forceinline__ void sample_node(const PassArgs& a, const NodeRec& r, i64 off, i64 pos0, i64 src_pos, i64 pbase,
                                             int g, int gl, int gbase, unsigned gmask) {
   const idx_t* __restrict__ col = (const idx_t*)a.col;
@@ -642,7 +638,6 @@ __device__ __forceinline__ void sample_node(const PassArgs& a, const NodeRec& r,
     a.eid[pbase + p] = e;
     a.colv[pbase + p] = d;  // global id for now; the (deferred) lookup overwrites it with the local id
     if (PHASED && a.phase == 3) return;   // distributed one-hop sampling: no mapping at all (neighbor_kernel.cpp:296-303)
-    if (PK) { a.eslot[p] = v2_insert(a.pk, a.pk_bits, (u32)d, (u32)p); return; }
     const u32 s = table_insert(a.keys, a.mask, make_key(d, sbatch, a.disjoint));
     red_min_u64(&a.vals[s], POS_BASE + (u64)p);
     a.eslot[p] = s;
@@ -662,9 +657,7 @@ __device__ __forceinline__ void sample_node(const PassArgs& a, const NodeRec& r,
 // nodes per warp, one wave) 33 us; 8 lanes with two draws per lane 34 us — more nodes in flight per SM lengthen
 // every gather / table insert more than the saved wave is worth, so the kernel stays with one draw per lane.
 inline int sample_group_lanes(i64 k) {
-  static const int exact = getenv("PYGB200_SAMPLE_EXACT_GROUPS") != nullptr;
   if (k < 0 || k > 16) return 32;
-  if (exact) return (int)(k < 1 ? 1 : k);
   return k > 8 ? 16 : (k > 4 ? 8 : 4);
 }
 inline int sample_nodes_per_block(int g) { return (NT / 32) * (32 / g); }
@@ -788,133 +781,6 @@ __global__ void __launch_bounds__(NT) k_mark(const PassArgs a) {
   }
 }
 
-// k_mark + k_assign in one launch (bounded, non-seed passes): tiles of 1024 edges are claimed in order
-// through a ticket; every tile publishes {epoch | status | value} — first its count of first occurrences
-// (status 1), then, after a decoupled look-back over the preceding tiles (warp 0, 32 tiles per step), its
-// inclusive prefix (status 2) — and assigns ids straight away.  The epoch makes stale words from earlier
-// launches invisible, so the tile array never needs clearing.  The block that finishes the last tile does
-// the counter / end-of-hop bookkeeping; ids_base / list_base are read before a block takes its first
-// ticket, i.e. strictly before the last tile can complete, so they are stable for every reader.
-__device__ __forceinline__ u64 tile_word(u32 epoch, u32 status, u32 value) {
-  return ((u64)epoch << 32) | ((u64)status << 30) | (u64)value;
-}
-__global__ void __launch_bounds__(NT) k_mark_assign(const PassArgs a, u32 epoch) {
-  __shared__ u32 s_w[NT / 32];
-  __shared__ i64 s_ticket;
-  __shared__ u32 s_excl;
-  pdl_enter();
-  const i64 E = a.st[ST_PASS_E], pbase = a.st[ST_PASS_BASE];
-  const i64 ids_base = a.st[a.o_dst_ids], list_base = a.st[a.o_dst_list];
-  const i64 ntiles = ceil_div(E, ETILE);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  volatile u64* tiles = reinterpret_cast<volatile u64*>(a.mtile);
-  u64* ticket = reinterpret_cast<u64*>(&a.st[ST_TICKET_B]);
-  while (true) {
-    __syncthreads();
-    if (threadIdx.x == 0) s_ticket = (i64)atomicAdd(ticket, 1ull);
-    __syncthreads();
-    const i64 tile = s_ticket;
-    if (tile >= ntiles) {
-      if (threadIdx.x == 0) {
-        if (tile == ntiles + (i64)gridDim.x - 1) *ticket = 0;   // the very last draw of this launch
-        if (ntiles == 0 && tile == 0) {                          // nothing emitted: only the bookkeeping remains
-          a.st[ST_PASS_NEW] = 0;
-          a.st[ST_LIST_BASE] = list_base; a.st[ST_IDS_BASE] = ids_base;
-        }
-      }
-      if (ntiles == 0 && tile == 0) {
-        __syncthreads();
-        for (int t = threadIdx.x; t < a.he_T; t += NT) {
-          const i64 n = a.st[a.he_list + t], e = a.st[a.he_end + t];
-          a.st[a.he_nph + t * (a.he_L + 1) + a.he_hop + 1] = n - e;
-          a.st[a.he_begin + t] = e;
-          a.st[a.he_end + t] = n;
-        }
-      }
-      break;
-    }
-    const i64 p0 = tile * ETILE + threadIdx.x * 4;
-    u32 fl[4], sl[4]; u32 cnt = 0;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const i64 p = p0 + q;
-      fl[q] = 0; sl[q] = 0;
-      if (p < E) { sl[q] = a.eslot[p]; fl[q] = (a.vals[sl[q]] == POS_BASE + (u64)p) ? 1u : 0u; }
-      cnt += fl[q];
-    }
-    u32 inc = cnt;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const u32 o = __shfl_up_sync(0xffffffffu, inc, d);
-      if (lane >= d) inc += o;
-    }
-    if (lane == 31) s_w[wid] = inc;
-    __syncthreads();
-    u32 pre = 0, tot = 0;
-    for (int w = 0; w < NT / 32; ++w) { if (w < wid) pre += s_w[w]; tot += s_w[w]; }
-    if (wid == 0) {
-      u32 excl = 0;
-      if (tile > 0) {
-        if (lane == 0) tiles[tile] = tile_word(epoch, 1, tot);
-        i64 base = tile - 1;
-        while (true) {
-          const i64 idx = base - lane;
-          u64 w = idx >= 0 ? tiles[idx] : tile_word(epoch, 2, 0);   // virtual tile -1: prefix 0
-          const bool valid = (u32)(w >> 32) == epoch && ((w >> 30) & 3u) != 0;
-          const bool is_pre = valid && ((w >> 30) & 3u) == 2;
-          const unsigned bv = __ballot_sync(0xffffffffu, valid), bp = __ballot_sync(0xffffffffu, is_pre);
-          const int first_pre = bp ? (__ffs(bp) - 1) : 32;          // nearest tile that already knows its prefix
-          const unsigned need = first_pre >= 31 ? 0xffffffffu : ((2u << first_pre) - 1u);
-          if ((bv & need) != need) continue;                        // somebody in range has not published yet: poll again
-          u32 v = (lane <= first_pre) ? (u32)(w & 0x3fffffffu) : 0u;
-#pragma unroll
-          for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
-          excl += v;
-          if (bp) break;
-          base -= 32;
-        }
-      }
-      if (lane == 0) {
-        __threadfence();
-        tiles[tile] = tile_word(epoch, 2, excl + tot);
-        s_excl = excl;
-      }
-    }
-    __syncthreads();
-    const u32 excl = s_excl;
-    u32 ex = excl + pre + inc - cnt;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      if (fl[q]) {
-        const i64 p = p0 + q;
-        const i64 rank = ex;
-        a.vals[sl[q]] = (u64)(ids_base + rank);
-        a.dst_nodes[list_base + rank] = a.colv[pbase + p];
-        if (a.disjoint) a.dst_batch[list_base + rank] = a.src_batch[a.row[pbase + p]];
-        a.dst_slot[list_base + rank] = sl[q];
-      }
-      ex += fl[q];
-    }
-    if (tile == ntiles - 1) {   // last tile: excl + tot == number of new nodes of the pass
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        const i64 nnew = (i64)excl + tot;
-        a.st[ST_PASS_NEW] = nnew;
-        a.st[ST_LIST_BASE] = list_base; a.st[ST_IDS_BASE] = ids_base;
-        a.st[a.o_dst_list] = list_base + nnew;
-        a.st[a.o_dst_ids] = ids_base + nnew;
-      }
-      __syncthreads();
-      for (int t = threadIdx.x; t < a.he_T; t += NT) {
-        const i64 n = a.st[a.he_list + t], e = a.st[a.he_end + t];
-        a.st[a.he_nph + t * (a.he_L + 1) + a.he_hop + 1] = n - e;
-        a.st[a.he_begin + t] = e;
-        a.st[a.he_end + t] = n;
-      }
-    }
-  }
-}
-
 __global__ void __launch_bounds__(NT) k_assign(const PassArgs a) {
   pdl_enter(TL_ASSIGN);
   const i64 E = a.st[ST_PASS_E];
@@ -1004,7 +870,7 @@ __global__ void __launch_bounds__(NT) k_count_s(const PassArgs a) {
   tl_mark(TL_COUNT | TL_END);
 }
 
-template <typename idx_t, bool PK = false>
+template <typename idx_t>
 __global__ void __launch_bounds__(NT, SAMPLE_MIN_BLOCKS) k_sample_s(const PassArgs a) {
   __shared__ u32 s_off[LAT_TILES], s_pos[LAT_TILES];
   __shared__ u32 s_win[MT_WIN];   // (block 0, stream shortfall only)
@@ -1097,7 +963,7 @@ __global__ void __launch_bounds__(NT, SAMPLE_MIN_BLOCKS) k_sample_s(const PassAr
     const i64 off = (i64)s_off[tile] + r.loc_off;
     const int ph = (int)(tpos & 3);
     const u32 pfv = ph == 0 ? rb.x : (ph == 1 ? rb.y : (ph == 2 ? rb.z : rb.w));
-    sample_node<idx_t, false, PK>(a, r, off, tpos + pfv, begin + i, pbase, g, gl, gbase, gmask);
+    sample_node<idx_t, false>(a, r, off, tpos + pfv, begin + i, pbase, g, gl, gbase, gmask);
   }
   tl_mark(TL_SAMPLE | TL_END);
 }
@@ -1178,118 +1044,6 @@ __global__ void __launch_bounds__(NT) k_assign_s(const PassArgs a) {
       if (a.disjoint) a.dst_batch[list_base + rank] = a.src_batch[a.row[pbase + p]];
       a.dst_slot[list_base + rank] = s;
     }
-  }
-}
-
-// ---- latency schedule on the PACKED table (runs that qualify for it: not disjoint, not temporal, node ids < 2^32 - 1):
-// the same write-once counters and per-block rescans as k_mark_s / k_assign_s, with sampler_v2.cuh's data path — one CAS
-// per insert in k_sample_s<PK>, refs read once in the mark kernel, ids from rank lookups, so an edge's local id is final
-// when the assign kernel stores it and no lookup of a pass is deferred into the next kernel any more.
-__global__ void __launch_bounds__(NT) k_mark_p(const PassArgs a) {
-  __shared__ u32 s_w[NT / 32];
-  pdl_enter(TL_MARK);
-  const i64 E = a.st[a.w_E];
-  const i64 ntiles = ceil_div(E, ETILE);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  u32 mine = 0;
-  for (i64 tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const i64 p0 = tile * ETILE + threadIdx.x * 4;
-    u32 fl[4], rv[4], cnt = 0;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) { const i64 p = p0 + q; rv[q] = p < E ? (u32)a.pk[a.eslot[p]] : 0u; }   // four independent chains
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const i64 p = p0 + q;
-      fl[q] = (p < E && rv[q] == (V2_POS | (u32)p)) ? 1u : 0u;
-      if (p < E) a.fref[p] = rv[q];
-      cnt += fl[q];
-    }
-    u32 inc = cnt;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const u32 o = __shfl_up_sync(0xffffffffu, inc, d);
-      if (lane >= d) inc += o;
-    }
-    if (lane == 31) s_w[wid] = inc;
-    __syncthreads();
-    u32 pre = 0, tot = 0;
-    for (int w = 0; w < NT / 32; ++w) { if (w < wid) pre += s_w[w]; tot += s_w[w]; }
-    u32 ex = pre + inc - cnt;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const i64 p = p0 + q;
-      if (p < E) a.erank[p] = ex;     // rank of p among the tile's firsts (only read for firsts)
-      ex += fl[q];
-    }
-    if (threadIdx.x == 0) { a.mtile[tile] = tot; mine += tot; }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0 && mine) atomicAdd(reinterpret_cast<unsigned long long*>(a.st + a.w_new), (unsigned long long)mine);
-  tl_mark(TL_MARK | TL_END);
-}
-
-__global__ void __launch_bounds__(NT) k_assign_p(const PassArgs a) {
-  __shared__ u32 s_excl[LAT_TILES];
-  __shared__ u32 s_w[NT / 32];
-  pdl_enter(TL_ASSIGN);
-  const i64 E = a.st[a.w_E];
-  const i64 pbase = ldw(a.st, a.w_pbase, 0);
-  const i64 list_base = ldw(a.st, a.w_list_in, a.c_list_in);
-  const i64 ids_base = list_base - (a.st[a.w_seed_list] - a.st[a.w_seed_ids]);   // duplicate seeds are listed, not numbered
-  const int ntiles = (int)ceil_div(E, ETILE);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (a.pub_words && blockIdx.x == 0 && threadIdx.x == 0) {   // last pass of the run: its dst list length was the last counter
-    publish_last(a, list_base + a.st[a.w_new]);
-    tl_mark(TL_FINAL);
-  }
-  const i64 p_first = (i64)blockIdx.x * NT + threadIdx.x;
-  u32 r_first = 0;
-  if (p_first < E) r_first = a.fref[p_first];
-  // ---- every block: exclusive scan of the per-tile counts of first occurrences
-  {
-    const int t0 = threadIdx.x * 4;
-    u32 pv[4]; u32 lv = 0;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int t = t0 + q;
-      pv[q] = lv;
-      if (t < ntiles) lv += (u32)a.mtile[t];
-    }
-    u32 inc = lv;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const u32 o = __shfl_up_sync(0xffffffffu, inc, d);
-      if (lane >= d) inc += o;
-    }
-    if (lane == 31) s_w[wid] = inc;
-    __syncthreads();
-    u32 pre = 0, tot = 0;
-    for (int w = 0; w < NT / 32; ++w) { if (w < wid) pre += s_w[w]; tot += s_w[w]; }
-    const u32 ex = pre + inc - lv;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int t = t0 + q;
-      if (t < ntiles) s_excl[t] = ex + pv[q];
-    }
-    if (blockIdx.x == 0 && threadIdx.x == 0) a.st[a.w_list_out] = list_base + tot;
-    __syncthreads();
-  }
-  for (i64 p = p_first; p < E; p += (i64)gridDim.x * NT) {
-    const u32 r = p == p_first ? r_first : a.fref[p];
-    i64 id = (i64)r;
-    if (r & V2_POS) {   // first seen in this pass, at position q: the rank of q among the pass's firsts
-      const u32 q = r & ~V2_POS;
-      const i64 rank = (i64)s_excl[q / ETILE] + (i64)__ldg(&a.erank[q]);
-      id = ids_base + rank;
-      if (q == (u32)p) {
-        const i64 d = a.colv[pbase + p];   // (global id, about to be replaced)
-        const u32 s = a.eslot[p];
-        a.dst_nodes[list_base + rank] = d;
-        a.dst_slot[list_base + rank] = s;
-        if (a.v2_writeback) a.pk[s] = ((u64)(u32)d << 32) | (u64)id;
-      }
-    }
-    a.colv[pbase + p] = id;
   }
 }
 
@@ -1390,12 +1144,10 @@ __global__ void __launch_bounds__(SEED_NT) k_seed_fused(const PassArgs a, const 
     }
     return;
   }
-  const bool packed = a.pk != nullptr;   // (latency schedule on the packed table: k_mark_p / k_assign_p)
   for (int i = threadIdx.x; i < n; i += SEED_NT) {
     const i64 v = (i64)seeds[i];
     a.dst_nodes[i] = v;
     if (a.disjoint) a.dst_batch[i] = batch0 + i;
-    if (packed) { a.eslot[i] = v2_insert(a.pk, a.pk_bits, (u32)v, (u32)i); continue; }
     const u32 s = table_insert(a.keys, a.mask, make_key(v, batch0 + i, a.disjoint));
     red_min_u64(&a.vals[s], POS_BASE + (u64)i);
     a.eslot[i] = s;
@@ -1407,7 +1159,7 @@ __global__ void __launch_bounds__(SEED_NT) k_seed_fused(const PassArgs a, const 
     u32 s = 0; int first = 0;
     if (i < n) {
       s = a.eslot[i];
-      first = packed ? ((u32)a.pk[s] == (V2_POS | (u32)i) ? 1 : 0) : ((a.vals[s] == POS_BASE + (u64)i) ? 1 : 0);
+      first = (a.vals[s] == POS_BASE + (u64)i) ? 1 : 0;
     }
     int inc = first;
 #pragma unroll
@@ -1422,8 +1174,7 @@ __global__ void __launch_bounds__(SEED_NT) k_seed_fused(const PassArgs a, const 
     const int c0 = s_carry;
     if (i < n) a.dst_slot[i] = first ? s : NO_SLOT;
     __syncthreads();   // every thread has read vals[] of this chunk before ranks overwrite them
-    if (first && packed) a.pk[s] = ((u64)(u32)a.dst_nodes[i] << 32) | (u64)(u32)(c0 + pre + inc - 1);
-    else if (first) a.vals[s] = (u64)(c0 + pre + inc - 1);
+    if (first) a.vals[s] = (u64)(c0 + pre + inc - 1);
     if (threadIdx.x == 0) s_carry = c0 + tot;
     __syncthreads();
   }
@@ -1586,7 +1337,6 @@ struct pygb200_sampler {
   i64* st_host = nullptr;   // pinned + mapped mirror of the state buffer (k_final writes it directly)
   i64* st_host_dev = nullptr;   // device-side address of st_host
   i64 run_serial = 0;       // completion flag value of the current run
-  unsigned epoch = 0;       // tag of the tile words of k_mark_assign launches
   bool cleanup_pending = false;   // the last run left its table reset to pygb200_sampler_export_all
   int st_o_list = 0;        // offset of the node-list counters inside `st` (for the deferred cleanup)
   // persistent mt19937 raw stream: survives between runs while torch's CPU generator is exactly where
@@ -1619,28 +1369,6 @@ struct pygb200_sampler {
   int T = 0, R = 0, L = 0;
   std::mutex mu;
 };
-
-// Debug: host-side time per segment of a run (PYGB200_HOST_TIMING=1, printed at exit)
-struct HostTimes {
-  bool on = getenv("PYGB200_HOST_TIMING") != nullptr;
-  double acc[6] = {0, 0, 0, 0, 0, 0};
-  double sub[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // finer laps inside "setup" (debug)
-  long runs = 0;
-  long branch[5] = {0, 0, 0, 0, 0};   // stream coverage at run start: known / older event / newer event / extend here / restart
-  static double now() { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-  ~HostTimes() {
-    if (on && runs)
-      fprintf(stderr, "[pygb200 host us/run over %ld runs] setup %.2f  mt+memset %.2f  seeds %.2f  hops+final %.2f  spin %.2f  post %.2f\n",
-              runs, acc[0] / runs, acc[1] / runs, acc[2] / runs, acc[3] / runs, acc[4] / runs, acc[5] / runs);
-    if (on && runs)
-      fprintf(stderr, "[pygb200 setup laps us/run] checks+bounds %.2f  schedule %.2f  direct+cleanup %.2f  layout+state %.2f  workspace %.2f\n",
-              sub[0] / runs, sub[1] / runs, sub[2] / runs, sub[3] / runs, sub[4] / runs);
-    if (on && runs)
-      fprintf(stderr, "[pygb200 mt19937 stream at run start] covered %ld  older event %ld  newer event %ld  extended here %ld  restarted %ld\n",
-              branch[0], branch[1], branch[2], branch[3], branch[4]);
-  }
-};
-static HostTimes g_ht;
 
 extern "C" const char* pygb200_last_error(void) { return g_err.c_str(); }
 extern "C" int pygb200_cuda_version(void) { return CUDART_VERSION; }
@@ -1856,16 +1584,15 @@ int ensure_edge_scratch(pygb200_sampler* s, i64 E, cudaStream_t st) {
   return PYGB200_OK;
 }
 
-// launch with the programmatic-stream-serialization attribute (see pdl_enter)
+// kernel<<<grid, block, smem, st>>>(args...) with the programmatic-stream-serialization attribute (see pdl_enter)
 template <typename... KP, typename... A>
-cudaError_t launch_pdl(void (*kernel)(KP...), int grid, int block, cudaStream_t st, A... args) {
-  static const bool off = getenv("PYGB200_NO_PDL") != nullptr;
+cudaError_t launch_pdl(void (*kernel)(KP...), dim3 grid, int block, size_t smem, cudaStream_t st, A... args) {
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3((unsigned)block); cfg.dynamicSmemBytes = 0; cfg.stream = st;
+  cfg.gridDim = grid; cfg.blockDim = dim3((unsigned)block); cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = off ? 0 : 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, KP(args)...);
 }
 
@@ -1902,16 +1629,17 @@ void load_jump_table(pygb200_sampler* s, cudaStream_t st) {
   }
 }
 
+// Jump-ahead has a fixed cost (~0.6 ms: serial pre-step + one polynomial pass per chunk); the one-CTA generator makes 2 G words/s
+// (measured with biased sampling, which asks for 10^5..10^8 words at a time): the crossover is at ~1.2 M words.
+constexpr i64 JUMP_MIN_WORDS = 1250000;
+
 // Queue generation of the raw stream up to (at least) `target` on `st`.  Large requests are split over
 // CTAs by jump-ahead (~20k-word serial pre-step + one pass over it per chunk), small ones run on one CTA.
 int mt_request(pygb200_sampler* s, cudaStream_t st, i64 target) {
   target = std::min<i64>(target, s->raw_cap_words - MT_N);
   while (target > s->mt_requested) {
     const i64 amount = target - s->mt_requested;
-    // jump-ahead has a fixed cost (~0.6 ms: serial pre-step + one polynomial pass per chunk); the one-CTA generator makes 2 G words/s
-    // (measured with biased sampling, which asks for 10^5..10^8 words at a time): the crossover is at ~1.2 M words
-    static const i64 jump_min = [] { const char* e = getenv("PYGB200_MT_JUMP_MIN_WORDS"); return e ? (i64)atoll(e) : (i64)1250000; }();
-    if (s->jump_P >= 2 && amount >= std::max<i64>(2 * (i64)s->jump_S, jump_min)) {
+    if (s->jump_P >= 2 && amount >= std::max<i64>(2 * (i64)s->jump_S, JUMP_MIN_WORDS)) {
       const int P_used = (int)std::min<i64>(s->jump_P, (amount + s->jump_S - 1) / s->jump_S);
       i64* jb = s->jump_scratch.as<i64>();
       k_mt_jump_prestep<3><<<1, 640, 0, st>>>(s->raw.as<u32>(), s->gen.as<i64>(), jb, s->raw_cap_words);
@@ -1937,7 +1665,7 @@ int launch_count(pygb200_sampler* s, const PassArgs& a, i64 F, i64 E_prev, cudaS
   // the grid also has to cover the deferred lookup of the previous pass (E_prev edges)
   const int g = std::max(grid_for(F, NT, s->sm_count), a.lk_colv ? grid_for(E_prev, NT, s->sm_count) : 1);
   void* tk = prof_begin(st);
-  launch_pdl(k_count<idx_t>, g, NT, st, a);
+  launch_pdl(k_count<idx_t>, g, NT, 0, st, a);
   prof_end(tk, "count", st, F);
   PYGB_LAUNCH_CHECK();
   return PYGB200_OK;
@@ -1949,7 +1677,7 @@ int launch_sample(pygb200_sampler* s, const PassArgs& a_in, i64 F, i64 E, cudaSt
   a.group = sample_group_lanes(a.fanout);
   const int gs = grid_for(F, sample_nodes_per_block(a.group), s->sm_count);
   void* tk = prof_begin(st);
-  launch_pdl(k_sample<idx_t>, gs, NT, st, a);
+  launch_pdl(k_sample<idx_t>, gs, NT, 0, st, a);
   prof_end(tk, "sample", st, E);
   PYGB_LAUNCH_CHECK();
   return PYGB200_OK;
@@ -1958,22 +1686,12 @@ int launch_sample(pygb200_sampler* s, const PassArgs& a_in, i64 F, i64 E, cudaSt
 template <typename idx_t>
 int launch_rest(pygb200_sampler* s, const PassArgs& a, i64 F, i64 E, bool lookup_now, cudaStream_t st, bool with_sample = true) {
   if (with_sample) if (int e = launch_sample<idx_t>(s, a, F, E, st)) return e;
-  // Opt-in (PYGB200_FUSE_MARK=1): mark + assign in one launch via decoupled look-back.  Measured on C2 it is a
-  // wash (94.6 vs 90.8 us per call): with PDL the kernel boundary it removes costs less than the look-back poll.
-  static const bool fuse = getenv("PYGB200_FUSE_MARK") != nullptr;
-  if (!lookup_now && !a.seed_mode && E < ((i64)1 << 30) && fuse) {
-    void* tk2 = prof_begin(st);
-    launch_pdl(k_mark_assign, grid_for(E, ETILE, s->sm_count), NT, st, a, (u32)(++s->epoch));
-    prof_end(tk2, "mark", st, E);
-    PYGB_LAUNCH_CHECK();
-    return PYGB200_OK;
-  }
   void* tk = prof_begin(st);
-  launch_pdl(k_mark, grid_for(E, ETILE, s->sm_count), NT, st, a);
+  launch_pdl(k_mark, grid_for(E, ETILE, s->sm_count), NT, 0, st, a);
   prof_end(tk, "mark", st, E);
   PYGB_LAUNCH_CHECK();
   tk = prof_begin(st);
-  launch_pdl(k_assign, grid_for(E, NT, s->sm_count), NT, st, a);
+  launch_pdl(k_assign, grid_for(E, NT, s->sm_count), NT, 0, st, a);
   prof_end(tk, "assign", st, E);
   PYGB_LAUNCH_CHECK();
   if (lookup_now) {
@@ -1996,10 +1714,6 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
   const bool bound_armed = s->bound.armed;
   s->bound.armed = false;
   s->last_direct = false;
-  double ht_last = g_ht.on ? HostTimes::now() : 0;
-  auto ht_lap = [&](int seg) { if (g_ht.on) { const double t = HostTimes::now(); g_ht.acc[seg] += t - ht_last; ht_last = t; } };
-  double ht_sub = ht_last;
-  auto sub_lap = [&](int seg) { if (g_ht.on) { const double t = HostTimes::now(); g_ht.sub[seg] += t - ht_sub; ht_sub = t; } };
   i64 total_seeds = 0;
   for (int t = 0; t < T; ++t) {
     PYGB_CHECK(n_seeds[t] >= 0, PYGB200_ERR_ARG, "negative seed count");
@@ -2085,7 +1799,6 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
                      "(exponential_), which this path does not reproduce");
   }
   if (mixed) synced = true;   // the host follows the engine's block count pass by pass
-  sub_lap(0);
   const bool sharded = shard != nullptr && shard->world > 1;
   const bool nodedup = (flags & PYGB200_S_NO_DEDUP) != 0;
   if (nodedup) PYGB_CHECK(T == 1 && R == 1 && L == 1 && !sharded, PYGB200_ERR_ARG,
@@ -2109,13 +1822,7 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
       lat = fb[(size_t)rels[r].src_type * (L + 1) + h] <= (i64)LAT_TILES * NT && eb[(size_t)r * L + h] <= (i64)LAT_TILES * ETILE;
     }
   const bool p2p = sharded && shard->exchange != nullptr;
-  // (PYGB200_LAT_PACKED=1: the latency schedule on the packed table — k_sample_s<PK> / k_mark_p / k_assign_p.  Measured on C2,
-  //  same box: 75.9-77.1 us per call against 73.8 on the wide table — at 1024 seeds the second-hop kernel is bound by its chain of
-  //  dependent loads, not by the two atomics per insert, and the side-stream table reset costs more host time than the lookup
-  //  it saves — so it stays opt-in)
-  static const bool no_lat_packed = getenv("PYGB200_LAT_PACKED") == nullptr;
-  bool v2 = !synced && !nodedup && !disjoint && !any_time && L > 0 && (!sharded || p2p) &&
-            (lat ? (!no_lat_packed && !no_v2) : (!no_v2 || p2p || weighted));
+  bool v2 = !lat && !synced && !nodedup && !disjoint && !any_time && L > 0 && (!sharded || p2p) && (!no_v2 || p2p || weighted);
   std::vector<i64> type_nodes((size_t)T, -1);   // nodes of each type, where a relation with that source type tells us
   for (int r = 0; r < R; ++r) type_nodes[rels[r].src_type] = std::max(type_nodes[rels[r].src_type], (i64)rels[r].num_src_nodes);
   if (v2)   // every node type's id range must be known and fit the packed key (a type that is never a source has no bound)
@@ -2125,7 +1832,6 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
   if (weighted) PYGB_CHECK(!sharded, PYGB200_ERR_UNSUPPORTED, "biased sampling is not frontier-sharded: one GPU per batch");
   const int XW = p2p ? shard->world : 1, XR = p2p ? shard->rank : 0;
 
-  sub_lap(1);
   // ---- results straight into the caller's arrays?  (bounded int64 non-disjoint runs only; the binding is one-shot)
   bool direct = bound_armed && !synced && (!sharded || shard->exchange != nullptr) && !nodedup && !idx32 && !disjoint &&
                 (int)s->bound.node.size() == T && (int)s->bound.row.size() == R;
@@ -2136,12 +1842,11 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
   // ---- workspace
   if (s->cleanup_pending && !s->types.empty() && s->types[0].tcap) {   // nobody exported the previous run: reset its table now
     auto& tb = s->types[0];
-    launch_pdl(k_cleanup, grid_for((i64)(tb.slot.cap / 4), NT, s->sm_count), NT, st, tb.keys.as<u64>(), tb.vals.as<u64>(),
+    launch_pdl(k_cleanup, grid_for((i64)(tb.slot.cap / 4), NT, s->sm_count), NT, 0, st, tb.keys.as<u64>(), tb.vals.as<u64>(),
                (const u32*)tb.slot.as<u32>(), (const i64*)(s->st_last + s->st_o_list));
     PYGB_LAUNCH_CHECK();
     s->cleanup_pending = false;
   }
-  sub_lap(2);
   if ((int)s->types.size() < T) s->types.resize(T);
   if ((int)s->rels.size() < R) s->rels.resize(R);
   s->T = T; s->R = R; s->L = L; s->disjoint = disjoint;
@@ -2161,7 +1866,6 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
     for (int i = 0; i < 2; ++i) PYGB_CUDA(cudaEventCreateWithFlags(&s->mt_ev[i], cudaEventDisableTiming));
     PYGB_CUDA(cudaEventCreateWithFlags(&s->mt_order_ev, cudaEventDisableTiming));
   }
-  sub_lap(3);
   if (s->dirty) {  // previous run aborted: wipe tables, forget the stream
     for (auto& tb : s->types) if (tb.tcap) {
       PYGB_CUDA(cudaMemsetAsync(tb.keys.p, 0xff, tb.tcap * 8, st));
@@ -2220,8 +1924,6 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
     if (int e = ensure_edge_scratch(s, total_seeds, st)) return e;
   }
 
-  sub_lap(4);
-  ht_lap(0);
   // ---- mt19937 raw stream: continue the persistent one or (re)start from the caller's engine state.
   // Pre-generation runs TWO runs ahead on the side stream: the launch made at the end of run i-1 already
   // covers run i+1, so in a steady loop this run only waits for an event that completed long ago while
@@ -2251,21 +1953,17 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
     const int older = s->mt_ev_next, newer = s->mt_ev_next ^ 1;
     if (s->mt_gen_known >= need) {
       // covered by a launch this stream has already waited for; newer launches keep running beside us
-      if (g_ht.on) g_ht.branch[0]++;
     } else if (s->mt_ev_pending[older] && s->mt_ev_target[older] >= need) {
-      if (g_ht.on) g_ht.branch[1]++;
       PYGB_CUDA(cudaStreamWaitEvent(st, s->mt_ev[older], 0));
       s->mt_ev_pending[older] = false;
       s->mt_gen_known = std::max(s->mt_gen_known, s->mt_ev_target[older]);
     } else if (s->mt_ev_pending[newer] && s->mt_ev_target[newer] >= need) {
-      if (g_ht.on) g_ht.branch[2]++;
       // same side stream: once the newer launch is complete so is the older one
       PYGB_CUDA(cudaStreamWaitEvent(st, s->mt_ev[newer], 0));
       s->mt_ev_pending[older] = s->mt_ev_pending[newer] = false;
       s->mt_gen_known = std::max(s->mt_gen_known, s->mt_ev_target[newer]);
     } else {
       // not covered ahead of time (first continued run, or a run larger than the previous one): extend here
-      if (g_ht.on) g_ht.branch[3]++;
       if (int e = wait_all_pregen()) return e;
       if (int e = mt_request(s, st, need)) return e;
       s->mt_gen_known = need;
@@ -2274,7 +1972,6 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
       PYGB_CUDA(cudaStreamWaitEvent(s->mt_stream, s->mt_order_ev, 0));
     }
   } else {
-    if (g_ht.on) g_ht.branch[4]++;
     if (int e = wait_all_pregen()) return e;
     static const i64 pref_cap = [] { const char* e = getenv("PYGB200_MT_CAP_WORDS"); return e ? (i64)atoll(e) : (i64)1 << 23; }();
     load_jump_table(s, st);
@@ -2375,11 +2072,9 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
   // Sharded: refs of owned positions -> barrier -> slice-wise reduction over the peers, result stored to all ->
   // barrier -> the same mark on the full ref array.  Then ids (replicated, streaming).
   static const u64 xbar_timeout_ns = [] { const char* e = getenv("PYGB200_XBARRIER_TIMEOUT_MS"); return (u64)(e ? atoll(e) : 20000) * 1000000ull; }();
-  static const int xfuse = [] { const char* e = getenv("PYGB200_XFUSE"); return e ? atoi(e) : 1; }();   // bit 0: flags raised by the last block of the producer kernel (default); bit 1: awaited by every block of the consumer (measured slower: 0.87 vs 0.76 ms at 2 GPUs)
-  auto xbarrier = [&](const PassArgs& a, int mode = 3) -> int {   // 1 = signal (opens a new epoch), 2 = wait for it, 3 = both
-    if (mode & 1) ++s->x.epoch;
+  auto xbarrier = [&](const PassArgs& a) -> int {   // wait until every rank has raised the flags of the current epoch
     void* tkb = prof_begin(st);
-    launch_pdl(k_xbarrier, 1, 32, st, a, (u64)s->x.epoch, xbar_timeout_ns, mode);
+    launch_pdl(k_xbarrier, 1, 32, 0, st, a, (u64)s->x.epoch, xbar_timeout_ns);
     prof_end(tkb, "xbarrier", st, 1);
     PYGB_LAUNCH_CHECK();
     return PYGB200_OK;
@@ -2389,38 +2084,28 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
     if (p2p) {
       PassArgs b = a;
       b.x_timeout_ns = xbar_timeout_ns;
-      if (xfuse & 1) b.x_sig_epoch = ++s->x.epoch;   // the last block of k_v2_exc raises the flags ...
+      b.x_sig_epoch = ++s->x.epoch;   // the last block of k_v2_exc raises the flags ...
       tk = prof_begin(st);
-      launch_pdl(k_v2_exc, grid_for(Eb, 4 * NT, s->sm_count), NT, st, b);
+      launch_pdl(k_v2_exc, grid_for(Eb, 4 * NT, s->sm_count), NT, 0, st, b);
       prof_end(tk, "pref", st, Eb);
       PYGB_LAUNCH_CHECK();
       b.x_sig_epoch = 0;
-      if (!(xfuse & 1)) if (int e = xbarrier(a, 1)) return e;
-      if (xfuse & 2) b.x_wait_epoch = s->x.epoch;    // ... k_v2_scatter waits for everybody's
-      else if (int e = xbarrier(a, 2)) return e;
+      if (int e = xbarrier(a)) return e;   // ... and k_v2_scatter starts behind everybody's
       tk = prof_begin(st);
-      {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)grid_for(ceil_div(Eb, XW), NT, s->sm_count), (unsigned)XW); cfg.blockDim = dim3(NT); cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        PYGB_CUDA(cudaLaunchKernelEx(&cfg, k_v2_scatter, b));
-      }
+      PYGB_CUDA(launch_pdl(k_v2_scatter, dim3((unsigned)grid_for(ceil_div(Eb, XW), NT, s->sm_count), (unsigned)XW), NT, 0, st, b));
       prof_end(tk, "reduce", st, Eb);
       PYGB_LAUNCH_CHECK();
       tk = prof_begin(st);
-      launch_pdl(k_v2_mark<false>, grid_for(Eb, ETILE, s->sm_count), NT, st, a);
+      launch_pdl(k_v2_mark<false>, grid_for(Eb, ETILE, s->sm_count), NT, 0, st, a);
     } else {
       tk = prof_begin(st);
-      launch_pdl(k_v2_mark<true>, grid_for(Eb, ETILE, s->sm_count), NT, st, a);
+      launch_pdl(k_v2_mark<true>, grid_for(Eb, ETILE, s->sm_count), NT, 0, st, a);
     }
     prof_end(tk, "mark", st, Eb);
     PYGB_LAUNCH_CHECK();
     tk = prof_begin(st);
-    if (p2p) launch_pdl(k_v2_assign<true>, grid_for(Eb, 4 * NT, s->sm_count), NT, st, a);
-    else launch_pdl(k_v2_assign<false>, grid_for(Eb, 4 * NT, s->sm_count), NT, st, a);
+    if (p2p) launch_pdl(k_v2_assign<true>, grid_for(Eb, 4 * NT, s->sm_count), NT, 0, st, a);
+    else launch_pdl(k_v2_assign<false>, grid_for(Eb, 4 * NT, s->sm_count), NT, 0, st, a);
     prof_end(tk, "assign", st, Eb);
     PYGB_LAUNCH_CHECK();
     return PYGB200_OK;
@@ -2451,7 +2136,7 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
   auto biased_count = [&](const PassArgs& a, i64 F_grid, i64 E_prev) -> int {
     const int g = std::max(grid_for(F_grid, NT, s->sm_count), a.lk_colv ? grid_for(E_prev, NT, s->sm_count) : 1);
     void* tk = prof_begin(st);
-    if (idx32) launch_pdl(k_w_count<int32_t>, g, NT, st, a); else launch_pdl(k_w_count<int64_t>, g, NT, st, a);
+    if (idx32) launch_pdl(k_w_count<int32_t>, g, NT, 0, st, a); else launch_pdl(k_w_count<int64_t>, g, NT, 0, st, a);
     prof_end(tk, "count", st, F_grid);
     PYGB_LAUNCH_CHECK();
     if (int e = read_state()) return e;
@@ -2494,13 +2179,8 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
       PYGB_CHECK(smem_ok, PYGB200_ERR_CUDA, "k_w_sample: cannot reserve shared memory for the candidate lists");
       const i64 kf = a.fanout;
       const size_t smem = (!a.replace && kf >= 0 && kf + 1 <= W_LIST_MAX) ? (size_t)(kf + 1) * (NT / 32) * 32 * 8 : 0;
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3((unsigned)gw); cfg.blockDim = dim3(NT); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[0].val.programmaticStreamSerializationAllowed = 1;
-      cfg.attrs = attr; cfg.numAttrs = 1;
-      if (idx32) PYGB_CUDA(cudaLaunchKernelEx(&cfg, k_w_sample<int32_t>, a, wa)); else PYGB_CUDA(cudaLaunchKernelEx(&cfg, k_w_sample<int64_t>, a, wa));
+      if (idx32) PYGB_CUDA(launch_pdl(k_w_sample<int32_t>, gw, NT, smem, st, a, wa));
+      else PYGB_CUDA(launch_pdl(k_w_sample<int64_t>, gw, NT, smem, st, a, wa));
     }
     prof_end(tk, "sample", st, E);
     PYGB_LAUNCH_CHECK();
@@ -2512,13 +2192,12 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
     if (int e = biased_draws(a, r)) return e;
     const i64 Eg = std::max<i64>(s->st_host[ST_PASS_E], 1);
     void* tk = prof_begin(st);
-    launch_pdl(k_v2_insert<false>, grid_for(Eg, 4 * NT, s->sm_count), NT, st, a);
+    launch_pdl(k_v2_insert<false>, grid_for(Eg, 4 * NT, s->sm_count), NT, 0, st, a);
     prof_end(tk, "insert", st, Eg);
     PYGB_LAUNCH_CHECK();
     return v2_ids(a, Eg);
   };
 
-  ht_lap(1);
   // ---- seeds (neighbor_kernel.cpp:409-416, :669-704)
   if (any_time) if (int e = s->seed_times.ensure((size_t)std::max<i64>(total_seeds, 1) * 8, 0, st)) return e;
   // The first pass that will run (hop 0) is counted inside the seed launch of its source type (extra blocks)
@@ -2552,25 +2231,25 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
       else k_seed_times<int64_t><<<g, NT, 0, st>>>(s->seed_times.as<i64>(), (const int64_t*)seeds[t], n_seeds[t], batch0, stt, ntt);
       PYGB_LAUNCH_CHECK();
     }
-    if (v2 && !lat) {
+    if (v2) {
       if (n_seeds[t] == 0) continue;   // the zeroed state already says "empty list, empty slice"
       if (p2p) { a.pk_main = a.pk; a.pk_main_bits = a.pk_bits; a.pk = s->seedpk[s->v2_side].as<u64>(); a.pk_bits = s->seedpk_bits[s->v2_side]; }
       a.sd_begin = lay.o_begin + t; a.sd_end = lay.o_end + t; a.sd_nph = lay.o_nph + t * (L + 1);   // (k_seed_end folded into the mark kernel)
       const int g = grid_for(n_seeds[t], NT, s->sm_count);
       void* tks = prof_begin(st);
-      if (idx32) launch_pdl(k_v2_seed<int32_t>, g, NT, st, a, (const int32_t*)seeds[t], (i64)n_seeds[t]);
-      else launch_pdl(k_v2_seed<int64_t>, g, NT, st, a, (const int64_t*)seeds[t], (i64)n_seeds[t]);
+      if (idx32) launch_pdl(k_v2_seed<int32_t>, g, NT, 0, st, a, (const int32_t*)seeds[t], (i64)n_seeds[t]);
+      else launch_pdl(k_v2_seed<int64_t>, g, NT, 0, st, a, (const int64_t*)seeds[t], (i64)n_seeds[t]);
       prof_end(tks, "seed", st, n_seeds[t]);
       PYGB_LAUNCH_CHECK();
       if (p2p) {
         // seeds: every rank dedups ALL of them in a scratch table of its own (65 k CAS, L2-resident) — no exchange, no
         // barrier; only the ids of the seeds a rank owns go into its partition of the real table (k_v2_assign)
         tks = prof_begin(st);
-        launch_pdl(k_v2_mark<true>, grid_for(n_seeds[t], ETILE, s->sm_count), NT, st, a);
+        launch_pdl(k_v2_mark<true>, grid_for(n_seeds[t], ETILE, s->sm_count), NT, 0, st, a);
         prof_end(tks, "mark", st, n_seeds[t]);
         PYGB_LAUNCH_CHECK();
         tks = prof_begin(st);
-        launch_pdl(k_v2_assign<true>, grid_for(n_seeds[t], 4 * NT, s->sm_count), NT, st, a);
+        launch_pdl(k_v2_assign<true>, grid_for(n_seeds[t], 4 * NT, s->sm_count), NT, 0, st, a);
         prof_end(tks, "assign", st, n_seeds[t]);
         PYGB_LAUNCH_CHECK();
         // (the scratch table is wiped on the side stream with this side's table reset, behind the run)
@@ -2578,9 +2257,9 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
       continue;
     }
     if (n_seeds[t] > 0 && n_seeds[t] <= SEED_FUSED_MAX) {
-      if (idx32) launch_pdl(k_seed_fused<int32_t>, 1 + count_blocks, SEED_NT, st, a, (const int32_t*)seeds[t], (int)n_seeds[t], batch0, (int)L,
+      if (idx32) launch_pdl(k_seed_fused<int32_t>, 1 + count_blocks, SEED_NT, 0, st, a, (const int32_t*)seeds[t], (int)n_seeds[t], batch0, (int)L,
                             lay.o_begin + t, lay.o_end + t, lay.o_nph + t * (L + 1), c);
-      else launch_pdl(k_seed_fused<int64_t>, 1 + count_blocks, SEED_NT, st, a, (const int64_t*)seeds[t], (int)n_seeds[t], batch0, (int)L,
+      else launch_pdl(k_seed_fused<int64_t>, 1 + count_blocks, SEED_NT, 0, st, a, (const int64_t*)seeds[t], (int)n_seeds[t], batch0, (int)L,
                       lay.o_begin + t, lay.o_end + t, lay.o_nph + t * (L + 1), c);
       PYGB_LAUNCH_CHECK();
     } else if (n_seeds[t] > 0) {
@@ -2588,16 +2267,15 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
       if (idx32) k_seed<int32_t><<<g, NT, 0, st>>>(a, (const int32_t*)seeds[t], n_seeds[t], batch0);
       else k_seed<int64_t><<<g, NT, 0, st>>>(a, (const int64_t*)seeds[t], n_seeds[t], batch0);
       PYGB_LAUNCH_CHECK();
-      launch_pdl(k_mark, grid_for(n_seeds[t], ETILE, s->sm_count), NT, st, a);
+      launch_pdl(k_mark, grid_for(n_seeds[t], ETILE, s->sm_count), NT, 0, st, a);
       PYGB_LAUNCH_CHECK();
-      launch_pdl(k_assign, g, NT, st, a);
+      launch_pdl(k_assign, g, NT, 0, st, a);
       PYGB_LAUNCH_CHECK();
       k_seed_end<<<1, 1, 0, st>>>(dst, t, L, lay.o_list, lay.o_begin, lay.o_end, lay.o_nph);
       PYGB_LAUNCH_CHECK();
     }  // n == 0: the zeroed state already says "empty list, empty slice"
   }
 
-  ht_lap(2);
   // ---- hops.  Bounded mode defers every pass's lookup into the next k_count / the final kernel.
   i64* lk_colv = nullptr; const u64* lk_vals = nullptr; i64 lk_E = 0;
   s->run_serial += 1;
@@ -2649,35 +2327,25 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
         if (!(h == 0 && r == fuse_r)) {   // (else: counted inside the seed launch)
           const int g = std::max(grid_for(Fb, NT, s->sm_count), lk_colv ? grid_for(lk_E, NT, s->sm_count) : 1);
           tk = prof_begin(st);
-          if (idx32) launch_pdl(k_count_s<int32_t>, g, NT, st, a); else launch_pdl(k_count_s<int64_t>, g, NT, st, a);
+          if (idx32) launch_pdl(k_count_s<int32_t>, g, NT, 0, st, a); else launch_pdl(k_count_s<int64_t>, g, NT, 0, st, a);
           prof_end(tk, "count", st, Fb);
           PYGB_LAUNCH_CHECK();
         }
         a.group = sample_group_lanes(k);
         const int gs = grid_for(Fb, sample_nodes_per_block(a.group), s->sm_count);
-        if (v2) {   // does any later pass insert into this dst type's table?  (else the ids need not be written back)
-          a.v2_writeback = 0;
-          for (int h2 = h; h2 < L && !a.v2_writeback; ++h2)
-            for (int r2 = (h2 == h ? r + 1 : 0); r2 < R && !a.v2_writeback; ++r2)
-              a.v2_writeback = rels[r2].dst_type == dst_t && num_neighbors[(size_t)r2 * L + h2] != 0 &&
-                               fb[(size_t)rels[r2].src_type * (L + 1) + h2] != 0 && eb[(size_t)r2 * L + h2] != 0;
-        }
         tk = prof_begin(st);
-        if (v2) { if (idx32) launch_pdl(k_sample_s<int32_t, true>, gs, NT, st, a); else launch_pdl(k_sample_s<int64_t, true>, gs, NT, st, a); }
-        else if (idx32) launch_pdl(k_sample_s<int32_t>, gs, NT, st, a); else launch_pdl(k_sample_s<int64_t>, gs, NT, st, a);
+        if (idx32) launch_pdl(k_sample_s<int32_t>, gs, NT, 0, st, a); else launch_pdl(k_sample_s<int64_t>, gs, NT, 0, st, a);
         prof_end(tk, "sample", st, Eb);
         PYGB_LAUNCH_CHECK();
         tk = prof_begin(st);
-        if (v2) launch_pdl(k_mark_p, grid_for(Eb, ETILE, s->sm_count), NT, st, a);
-        else launch_pdl(k_mark_s, grid_for(Eb, ETILE, s->sm_count), NT, st, a);
+        launch_pdl(k_mark_s, grid_for(Eb, ETILE, s->sm_count), NT, 0, st, a);
         prof_end(tk, "mark", st, Eb);
         PYGB_LAUNCH_CHECK();
         tk = prof_begin(st);
-        if (v2) launch_pdl(k_assign_p, grid_for(Eb, NT, s->sm_count), NT, st, a);
-        else launch_pdl(k_assign_s, grid_for(Eb, NT, s->sm_count), NT, st, a);
+        launch_pdl(k_assign_s, grid_for(Eb, NT, s->sm_count), NT, 0, st, a);
         prof_end(tk, "assign", st, Eb);
         PYGB_LAUNCH_CHECK();
-        if (!v2) { lk_colv = a.colv; lk_vals = a.vals; lk_E = Eb; lk_w_E = base; lk_w_pbase = relcum[r].w; }   // (packed: ids are final)
+        lk_colv = a.colv; lk_vals = a.vals; lk_E = Eb; lk_w_E = base; lk_w_pbase = relcum[r].w;
         cursor = Wd{base + 1, 0}; relcum[r] = Wd{base + 2, 0}; cur_list[dst_t] = Wd{base + 3, 0};
         eph_w[(size_t)r * L + h] = base;
       }
@@ -2734,47 +2402,34 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
           void* tk = prof_begin(st);
           if (p2p) {
             // (the positions of the ranks' frontier slices were written by the last block of k_count)
-            if (idx32) launch_pdl(k_v2_sample<int32_t, true>, gs, NT, st, a); else launch_pdl(k_v2_sample<int64_t, true>, gs, NT, st, a);
+            if (idx32) launch_pdl(k_v2_sample<int32_t, true>, gs, NT, 0, st, a); else launch_pdl(k_v2_sample<int64_t, true>, gs, NT, 0, st, a);
             prof_end(tk, "sample", st, Eb);
             PYGB_LAUNCH_CHECK();
             // own slice -> every peer with 16-byte stores; its last block raises this rank's flag at the peers ("my slice
             // has been delivered"), so the peers' flags arrive while the rows are written and k_v2_insert only has to look
             a.x_timeout_ns = xbar_timeout_ns;
-            if (xfuse & 1) a.x_sig_epoch = ++s->x.epoch;
+            a.x_sig_epoch = ++s->x.epoch;
             tk = prof_begin(st);
-            launch_pdl(k_v2_push, grid_for(ceil_div(Eb, XW) + 1, 4 * NT, s->sm_count), NT, st, a);
+            launch_pdl(k_v2_push, grid_for(ceil_div(Eb, XW) + 1, 4 * NT, s->sm_count), NT, 0, st, a);
             prof_end(tk, "push", st, Eb);
             PYGB_LAUNCH_CHECK();
             a.x_sig_epoch = 0;
-            if (!(xfuse & 1)) if (int e = xbarrier(a, 1)) return e;
             tk = prof_begin(st);
-            launch_pdl(k_v2_rows, grid_for(Fb, NT, s->sm_count), NT, st, a);
+            launch_pdl(k_v2_rows, grid_for(Fb, NT, s->sm_count), NT, 0, st, a);
             prof_end(tk, "rows", st, Eb);
             PYGB_LAUNCH_CHECK();
           } else {
-            // A/B switch: draws and table inserts in one kernel (default) or the inserts in an edge-parallel kernel of their
-            // own with four CAS in flight per thread (PYGB200_V2_SPLIT_INSERT=1)
-            static const bool split_insert = getenv("PYGB200_V2_SPLIT_INSERT") != nullptr;
-            if (split_insert) a.phase = 4;
-            if (idx32) launch_pdl(k_v2_sample<int32_t, false>, gs, NT, st, a); else launch_pdl(k_v2_sample<int64_t, false>, gs, NT, st, a);
+            // draws and table inserts in one kernel
+            if (idx32) launch_pdl(k_v2_sample<int32_t, false>, gs, NT, 0, st, a); else launch_pdl(k_v2_sample<int64_t, false>, gs, NT, 0, st, a);
             prof_end(tk, "sample", st, Eb);
             PYGB_LAUNCH_CHECK();
-            if (split_insert) {
-              void* tki = prof_begin(st);
-              launch_pdl(k_v2_insert<false>, grid_for(Eb, 4 * NT, s->sm_count), NT, st, a);
-              prof_end(tki, "insert", st, Eb);
-              PYGB_LAUNCH_CHECK();
-              a.phase = 0;
-            }
           }
           if (p2p) {
-            if (xfuse & 2) a.x_wait_epoch = s->x.epoch;   // every block first waits until everybody's (dst, edge id) have arrived
-            else if (int e = xbarrier(a, 2)) return e;
+            if (int e = xbarrier(a)) return e;   // until everybody's (dst, edge id) have arrived
             void* tki = prof_begin(st);
-            launch_pdl(k_v2_insert<true>, grid_for(Eb, 4 * NT, s->sm_count), NT, st, a);
+            launch_pdl(k_v2_insert<true>, grid_for(Eb, 4 * NT, s->sm_count), NT, 0, st, a);
             prof_end(tki, "insert", st, Eb);
             PYGB_LAUNCH_CHECK();
-            a.x_wait_epoch = 0;
           }
           if (int e = v2_ids(a, Eb)) return e;
           if (p2p) s->x.passes += 1;
@@ -2913,7 +2568,7 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
     }
     a.pub_wwords = wwords;
     void* tkf = prof_begin(st);
-    launch_pdl(k_final, lk_colv ? grid_for(lk_E, NT, s->sm_count) : 1, NT, st, a);
+    launch_pdl(k_final, lk_colv ? grid_for(lk_E, NT, s->sm_count) : 1, NT, 0, st, a);
     prof_end(tkf, "final", st, 1);
     PYGB_LAUNCH_CHECK();
   }
@@ -2927,7 +2582,7 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
   for (int t = 0; t < T && !s->cleanup_pending && !v2; ++t) {
     auto& tb = s->types[t];
     const i64 cap_nodes = (i64)(tb.slot.cap / 4);
-    launch_pdl(k_cleanup, grid_for(synced ? cap_nodes : node_cap[t], NT, s->sm_count), NT, st, tb.keys.as<u64>(), tb.vals.as<u64>(),
+    launch_pdl(k_cleanup, grid_for(synced ? cap_nodes : node_cap[t], NT, s->sm_count), NT, 0, st, tb.keys.as<u64>(), tb.vals.as<u64>(),
                (const u32*)tb.slot.as<u32>(), (const i64*)(dst + (lat && cur_list[t].w >= 0 ? cur_list[t].w : lay.o_list + t)));
     PYGB_LAUNCH_CHECK();
   }
@@ -2943,7 +2598,6 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
     }
     s->mt_defer_target = 0;
   }
-  ht_lap(3);
   {  // wait for k_final's flag (spin on mapped memory; keep an eye on the stream in case the run died)
     volatile i64* flag = s->st_host + lay.words;
     unsigned long long spins = 0;
@@ -2963,7 +2617,6 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
     }
     std::atomic_thread_fence(std::memory_order_acquire);
   }
-  ht_lap(4);
   if (pub_w_list >= 0) s->st_host[pub_w_list] = (i64)((u64)s->st_host[lay.words] & 0xffffffffffull);
   const i64* hs = s->st_host;
   PYGB_CHECK(hs[ST_ERROR] != 2, PYGB200_ERR_INTERNAL, "sampler: a peer rank did not reach a cross-GPU barrier in time (frontier-sharded run; PYGB200_XBARRIER_TIMEOUT_MS)");
@@ -3033,8 +2686,6 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
     // next run (see above) so that it costs no host time between two runs
     s->mt_defer_target = target > s->mt_q ? target : 0;
   }
-  ht_lap(5);
-  if (g_ht.on) g_ht.runs += 1;
   return PYGB200_OK;
 }
 
@@ -3200,10 +2851,10 @@ extern "C" int pygb200_sampler_export_all(pygb200_sampler* s, int32_t rel, void*
   const i64* node = s->types[type].nodes.as<i64>();
   const i64* batch = s->disjoint ? s->types[type].batch.as<i64>() : nullptr;
   if (index32)
-    launch_pdl(k_export4<int32_t>, g, NT, st, s0, s1, s2, (int32_t*)row_out, (int32_t*)col_out, (int32_t*)edge_id_out, ne, node,
+    launch_pdl(k_export4<int32_t>, g, NT, 0, st, s0, s1, s2, (int32_t*)row_out, (int32_t*)col_out, (int32_t*)edge_id_out, ne, node,
                batch, (int32_t*)node_id_out, nn, ck, cv, cs);
   else
-    launch_pdl(k_export4<int64_t>, g, NT, st, s0, s1, s2, (int64_t*)row_out, (int64_t*)col_out, (int64_t*)edge_id_out, ne, node,
+    launch_pdl(k_export4<int64_t>, g, NT, 0, st, s0, s1, s2, (int64_t*)row_out, (int64_t*)col_out, (int64_t*)edge_id_out, ne, node,
                batch, (int64_t*)node_id_out, nn, ck, cv, cs);
   PYGB_LAUNCH_CHECK();
   return PYGB200_OK;

@@ -35,15 +35,15 @@ __device__ __forceinline__ int v2_owner(u32 key, int W) {
 // insert (key, position p of the running pass); returns the slot.  The slot's value ends up as the minimum position
 // of the key in this pass, or stays the local id the key got in an earlier pass (ids < V2_POS <= positions).
 __device__ __forceinline__ u32 v2_insert(u64* __restrict__ pk, int bits, u32 key, u32 p) {
-  const u64 mask = (1ull << bits) - 1;
-  u64 s = ((u64)key * 0x9E3779B97F4A7C15ull) >> (64 - bits);
+  const u32 mask = (u32)((1ull << bits) - 1);   // (bits <= 32)
+  u32 s = (u32)(((u64)key * 0x9E3779B97F4A7C15ull) >> (64 - bits));
   const u64 mine = ((u64)key << 32) | (u64)(V2_POS | p);
   while (true) {
     const u64 prev = atomicCAS(&pk[s], EMPTY, mine);
-    if (prev == EMPTY) return (u32)s;
+    if (prev == EMPTY) return s;
     if ((u32)(prev >> 32) == key) {
       if ((u32)prev > (V2_POS | p)) red_min_u64(&pk[s], mine);
-      return (u32)s;
+      return s;
     }
     s = (s + 1) & mask;
   }
@@ -52,22 +52,22 @@ __device__ __forceinline__ u32 v2_insert(u64* __restrict__ pk, int bits, u32 key
 template <typename T>
 __device__ __forceinline__ T* x_ptr(const PassArgs& a, int q, i64 off) { return reinterpret_cast<T*>(a.xpeer[q] + off); }
 
-// ---- cross-GPU barrier on flag words in the exchange regions.  Stream order puts it behind the kernel whose peer
-// stores it publishes (a completed kernel's stores are performed system-wide); thread q tells rank q "rank xr has
-// reached epoch" and waits for rank q's word in its own region.  A peer that never arrives is reported, not waited
+// ---- cross-GPU barrier on flag words in the exchange regions.  The last block of a kernel that stored to the peers
+// tells every rank q "rank xr has reached epoch" (x_signal after last_block_sys); k_xbarrier, launched behind a kernel
+// that needs nothing remote where there is one (k_v2_rows), waits for every rank's word in its own region, so the
+// peers' skew hides behind local work.  Thread q waits for rank q.  A peer that never arrives is reported, not waited
 // for forever.
-// `mode`: 1 = signal only, 2 = wait only, 3 = both — a signal right behind the kernel that stored to the peers and the
-// wait after a kernel that needs nothing remote (k_v2_rows) hide the peers' skew behind local work.
-__global__ void k_xbarrier(const PassArgs a, u64 epoch, u64 timeout_ns, int mode) {
+__device__ __forceinline__ void x_signal(const PassArgs& a) {
+  if ((int)threadIdx.x < a.xw && (int)threadIdx.x != a.xr)
+    asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(x_ptr<u64>(a, threadIdx.x, a.x_off_bar) + a.xr), "l"(a.x_sig_epoch) : "memory");
+}
+__global__ void k_xbarrier(const PassArgs a, u64 epoch, u64 timeout_ns) {
   pdl_enter();
   const int q = threadIdx.x;
   if (q >= a.xw) return;
   __threadfence_system();
   u64* mine = x_ptr<u64>(a, a.xr, a.x_off_bar);
   if (q != a.xr) {
-    u64* theirs = x_ptr<u64>(a, q, a.x_off_bar);
-    if (mode & 1) asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(theirs + a.xr), "l"(epoch) : "memory");
-    if (!(mode & 2)) return;
     u64 t0, t1, v;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
     while (true) {
@@ -79,28 +79,6 @@ __global__ void k_xbarrier(const PassArgs a, u64 epoch, u64 timeout_ns, int mode
     }
   }
   __threadfence_system();
-}
-
-// the same flags, raised by the last block of a kernel that stored to the peers (x_signal after last_block_sys) and
-// awaited by every block of the kernel that consumes what arrived (x_wait at its start): no barrier launches at all
-__device__ __forceinline__ void x_signal(const PassArgs& a) {
-  if ((int)threadIdx.x < a.xw && (int)threadIdx.x != a.xr)
-    asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(x_ptr<u64>(a, threadIdx.x, a.x_off_bar) + a.xr), "l"(a.x_sig_epoch) : "memory");
-}
-__device__ __forceinline__ void x_wait(const PassArgs& a) {
-  if ((int)threadIdx.x < a.xw && (int)threadIdx.x != a.xr) {
-    const u64* mine = x_ptr<u64>(a, a.xr, a.x_off_bar) + threadIdx.x;
-    u64 t0, t1, v;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-    while (true) {
-      asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(mine) : "memory");
-      if (v >= a.x_wait_epoch) break;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-      if (t1 - t0 > a.x_timeout_ns) { a.st[ST_ERROR] = 2; break; }
-      __nanosleep(100);
-    }
-  }
-  __syncthreads();
 }
 
 // ---- seeds: list them and insert them at position i (first-occurrence order == seed order)
@@ -200,10 +178,10 @@ __global__ void __launch_bounds__(NT, SAMPLE_MIN_BLOCKS) k_v2_sample(const PassA
       const i64 p = off + j;
       const i64 d = (i64)col[e];
       if (!SH) {
+        a.eslot[p] = v2_insert(a.pk, a.pk_bits, (u32)d, (u32)p);
+        a.colv[pbase + p] = d;   // global id until k_v2_assign replaces it with the local id
         a.row[pbase + p] = src_pos;
         a.eid[pbase + p] = e;
-        a.colv[pbase + p] = d;   // global id until k_v2_assign replaces it with the local id
-        if (a.phase != 4) a.eslot[p] = v2_insert(a.pk, a.pk_bits, (u32)d, (u32)p);   // (phase 4: k_v2_insert<false> follows)
       } else {
         // into this rank's OWN exchange region; k_v2_push forwards the slice to the peers with wide, fully coalesced
         // stores — 4-byte lane stores straight to 7 peers made this kernel 227 us at 8 ranks for 1/8 of the draws
@@ -223,15 +201,13 @@ __global__ void __launch_bounds__(NT, SAMPLE_MIN_BLOCKS) k_v2_sample(const PassA
 // ---- sharded: the owner of a dst id inserts it (all positions of the pass are streamed, 1/W of them hit the table).
 // Four positions per thread (coalesced, strided by the block) with their first CAS issued back to back: the kernel is
 // bound by the round trips of independent atomics, not by their number.
-template <bool SH>   // SH = false: single GPU with the insert split from the draws (keys = the global ids in colv)
+template <bool SH>   // SH = false: single GPU, the inserts of a biased pass (keys = the global ids in colv)
 __global__ void __launch_bounds__(NT) k_v2_insert(const PassArgs a) {
   pdl_enter();
   const i64 E = a.st[ST_PASS_E];
   const i64 pbase = a.st[ST_PASS_BASE];
   const u32* __restrict__ xdst = SH ? x_ptr<u32>(a, a.xr, a.x_off_dst) : nullptr;
   const u64 mask = (1ull << a.pk_bits) - 1;
-  if (SH && a.x_wait_epoch) x_wait(a);
-  if (SH && blockIdx.x == 0 && threadIdx.x == 0) *x_ptr<u64>(a, a.xr, a.x_off_xcnt) = 0;   // this pass's exception count (k_v2_exc)
   for (i64 base = (i64)blockIdx.x * (4 * NT); base < E; base += (i64)gridDim.x * (4 * NT)) {
     u32 key[4]; u64 slot[4], prev[4]; bool own[4];
 #pragma unroll
@@ -266,6 +242,7 @@ __global__ void __launch_bounds__(NT) k_v2_insert(const PassArgs a) {
       if (SH) a.fref[p] = V2_POS | (u32)p;   // default ref "first occurrence"; the owners send the exceptions (k_v2_exc)
     }
   }
+  if (SH && blockIdx.x == 0 && threadIdx.x == 0) *x_ptr<u64>(a, a.xr, a.x_off_xcnt) = 0;   // this pass's exception count (k_v2_exc)
 }
 
 // ---- sharded: the refs every rank needs.  A position's ref is "first occurrence" (V2_POS | p, what k_v2_insert wrote
@@ -312,7 +289,6 @@ __global__ void __launch_bounds__(NT) k_v2_exc(const PassArgs a) {
 // blockIdx.y = source rank
 __global__ void __launch_bounds__(NT) k_v2_scatter(const PassArgs a) {
   pdl_enter();
-  if (a.x_wait_epoch) x_wait(a);
   const int sr = blockIdx.y;
   const i64 n = (i64)x_ptr<u64>(a, a.xr, a.x_off_exc_n)[sr];
   const u64* __restrict__ list = x_ptr<u64>(a, a.xr, a.x_off_exc) + (i64)sr * a.x_exc_cap;

@@ -13,7 +13,6 @@
 #include <memory>
 #include <mutex>
 
-#include <chrono>
 #include "common.h"
 
 namespace pyg {
@@ -27,20 +26,6 @@ typedef std::tuple<std::string, std::string, std::string> edge_type;
 inline rel_type to_rel_type(const edge_type& k) {  // pyg_lib/csrc/utils/types.h:10-12
   return std::get<0>(k) + "__" + std::get<1>(k) + "__" + std::get<2>(k);
 }
-
-// Debug: host time of the homogeneous op outside the ABI run (PYGB200_HOST_TIMING=1, printed at exit)
-struct OpTimes {
-  bool on = getenv("PYGB200_HOST_TIMING") != nullptr;
-  double pre = 0, run = 0, post = 0, between = 0, last_exit = 0;
-  long calls = 0;
-  static double now() { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-  ~OpTimes() {
-    if (on && calls)
-      fprintf(stderr, "[pygb200 op us/call over %ld calls] before run %.2f  run %.2f  after run %.2f  between calls (python+dispatcher) %.2f\n",
-              calls, pre / calls, run / calls, post / calls, between / (calls > 1 ? calls - 1 : 1));
-  }
-};
-static OpTimes g_ot;
 
 // one persistent workspace per (device, stream).  An op binds outputs, runs and exports in separate ABI calls, and torch
 // drops the GIL inside ops: `op_mu` is held across the whole op body so that two host threads sampling on the same
@@ -142,9 +127,6 @@ neighbor_sample_cuda(const at::Tensor& rowptr, const at::Tensor& col, const at::
                      const std::optional<at::Tensor>& edge_time, const std::optional<at::Tensor>& seed_time,
                      const std::optional<at::Tensor>& edge_weight, bool csc, bool replace, bool directed,
                      bool disjoint, std::string temporal_strategy, bool return_edge_id) {
-  const double ot0 = g_ot.on ? OpTimes::now() : 0;
-  double ot1 = 0, ot2 = 0;
-  if (g_ot.on && g_ot.calls) g_ot.between += ot0 - g_ot.last_exit;
   TORCH_CHECK(temporal_strategy == "uniform" || temporal_strategy == "last", "No valid temporal strategy found");
   check_arguments(node_time.has_value(), edge_time.has_value(), seed_time.has_value(), edge_weight.has_value(), disjoint);
   TORCH_CHECK(seed.is_cuda(), "pyg_lib_b200: neighbor_sample expects CUDA tensors (no CPU fallback)");
@@ -200,7 +182,6 @@ neighbor_sample_cuda(const at::Tensor& rowptr, const at::Tensor& col, const at::
     if (edge_weight.has_value() && std::any_of(num_neighbors.begin(), num_neighbors.end(), [](int64_t k) { return k >= 0; }))
       wp = weight_ptr(*edge_weight, col, seed.device());
     CpuEngine eng;
-    if (g_ot.on) ot1 = OpTimes::now();
     if (wp) {
       PYGB_TORCH_CALL(pygb200_sampler_run_weighted(s, 1, 1, L, &rel, seeds, &n_seed, num_neighbors.data(), flags, &eng.mt,
                                                    nph.data(), eph.data(), &n_nodes, &n_edges, stream, &wp, PYGB200_F32));
@@ -208,7 +189,6 @@ neighbor_sample_cuda(const at::Tensor& rowptr, const at::Tensor& col, const at::
     PYGB_TORCH_CALL(pygb200_sampler_run_temporal(s, 1, 1, L, &rel, seeds, &n_seed, num_neighbors.data(), flags, &eng.mt,
                                                  nph.data(), eph.data(), &n_nodes, &n_edges, stream,
                                                  (nt || et) ? &tmp : nullptr));
-    if (g_ot.on) ot2 = OpTimes::now();
     eng.commit();
   }
   TORCH_CHECK(directed, "Undirected subgraphs not yet supported");  // raised after sampling, neighbor_kernel.cpp:501
@@ -230,10 +210,6 @@ neighbor_sample_cuda(const at::Tensor& rowptr, const at::Tensor& col, const at::
                                                node.data_ptr(), idx32, stream));
   }
   if (csc) std::swap(row, colv);  // neighbor_kernel.cpp:155-159
-  if (g_ot.on) {
-    const double t = OpTimes::now();
-    g_ot.pre += ot1 - ot0; g_ot.run += ot2 - ot1; g_ot.post += t - ot2; g_ot.last_exit = t; g_ot.calls += 1;
-  }
   return std::make_tuple(row, colv, node, eid, nph, eph);
 }
 

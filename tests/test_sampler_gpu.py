@@ -440,9 +440,7 @@ print('OK', n)
 ''' % (ROOT, ROOT, ROOT)
     # (without the latency path bounded non-disjoint runs take the v2 schedule — packed table, refs — and the rest
     #  the wide-table throughput path; PYGB200_NO_V2 sends everything to the latter)
-    # (PYGB200_LAT_PACKED: the opt-in latency schedule on the packed table)
-    for extra in ({'PYGB200_NO_LATENCY_PATH': '1'}, {'PYGB200_DIRECT_OUTPUT_MB': '0'}, {'PYGB200_LAT_PACKED': '1'},
-                  {'PYGB200_LAT_PACKED': '1', 'PYGB200_DIRECT_OUTPUT_MB': '0'},
+    for extra in ({'PYGB200_NO_LATENCY_PATH': '1'}, {'PYGB200_DIRECT_OUTPUT_MB': '0'},
                   {'PYGB200_NO_LATENCY_PATH': '1', 'PYGB200_DIRECT_OUTPUT_MB': '0'},
                   {'PYGB200_NO_LATENCY_PATH': '1', 'PYGB200_NO_V2': '1'},
                   {'PYGB200_NO_LATENCY_PATH': '1', 'PYGB200_NO_V2': '1', 'PYGB200_DIRECT_OUTPUT_MB': '0'}):
