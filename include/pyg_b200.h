@@ -333,6 +333,18 @@ int pygb200_segment_gather(pygb200_subgraph* h, const void* const* src_ptrs_host
                            const int64_t* seg_begin_host, const int64_t* seg_count_host, int64_t n_seg, int broadcast,
                            int index32, void* out, void* stream);
 
+/* ------------------------------------------------------------------------------------ random walk
+ * Uniform random walks (pyg::random_walk with p == q == 1; replaces random_walk_kernel,
+ * pyg_lib/csrc/sampler/cuda/random_walk_kernel.cu:27-85).  rowptr [num_nodes + 1] / col [num_edges] / seed [S] of one
+ * index dtype (index32 != 0: int32, else int64); rand [walk_length, S] float32 draws in [0, 1), row-major (the caller
+ * fills it, e.g. with at::rand, so the generator is consumed exactly as the reference consumes it); out [S, walk_length + 1]
+ * row-major in the index dtype.  out[i][0] = seed[i]; step j moves v to col[rowptr[v] + min(int(rand[j][i] * float(deg)),
+ * deg - 1)] when deg = rowptr[v+1] - rowptr[v] > 0 and stays on v otherwise.  One kernel launch, no host sync.  A node
+ * index outside [0, num_nodes) in seed / col, or a row outside [0, num_edges), is never dereferenced: that walk stops
+ * there and the NEXT call returns PYGB200_ERR_ARG (the output of the call that met it is undefined). */
+int pygb200_random_walk(const void* rowptr, const void* col, int64_t num_nodes, int64_t num_edges, const void* seed,
+                        int64_t S, int64_t walk_length, const float* rand, void* out, int index32, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

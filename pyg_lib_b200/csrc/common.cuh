@@ -92,4 +92,10 @@ struct AsyncScratch {
 
 __host__ __device__ inline i64 ceil_div(i64 a, i64 b) { return (a + b - 1) / b; }
 
+// Asynchronous argument errors (matmul.cu): a kernel that finds invalid input raises its slot's flag instead of touching
+// memory, and the next call of that family reports it.  async_error_flag_dev may return null (no mapped memory).
+enum { ASYNC_ERR_MATMUL = 0, ASYNC_ERR_RANDOM_WALK = 1, ASYNC_ERR_SLOTS = 2 };
+int* async_error_flag_dev(int slot);
+bool take_async_error(int slot);   // reads and clears the slot's flag
+
 }  // namespace pygb200

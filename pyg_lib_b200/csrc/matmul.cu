@@ -38,23 +38,26 @@ int grouped_matmul_tc(const pygb200_gemm_problem* ps, i64 count, int dtype, cuda
 // `ptr` while they read it (ptr[0] == 0, non-decreasing, ptr[B] == N — what the reference's split_with_sizes checks on
 // the host after its D2H copy, matmul_kernel.cu:307) and raise the flag instead of touching memory; the NEXT matmul
 // call on this process reports it (like CUDA's own asynchronous errors), so a device-resident ptr still costs no sync.
+// random_walk.cu raises its own slot of the same allocation for node indices outside the graph.
 static int* g_mm_err_host = nullptr;
 static int* g_mm_err_dev = nullptr;
-int* mm_error_flag_dev() {
+int* async_error_flag_dev(int slot) {
   static bool tried = false;
   if (!tried) {
     tried = true;
-    if (cudaHostAlloc((void**)&g_mm_err_host, sizeof(int), cudaHostAllocMapped | cudaHostAllocPortable) == cudaSuccess) {
-      *g_mm_err_host = 0;
+    if (cudaHostAlloc((void**)&g_mm_err_host, ASYNC_ERR_SLOTS * sizeof(int), cudaHostAllocMapped | cudaHostAllocPortable) == cudaSuccess) {
+      for (int s = 0; s < ASYNC_ERR_SLOTS; ++s) g_mm_err_host[s] = 0;
       if (cudaHostGetDevicePointer((void**)&g_mm_err_dev, g_mm_err_host, 0) != cudaSuccess) g_mm_err_dev = nullptr;
     }
   }
-  return g_mm_err_dev;
+  return g_mm_err_dev ? g_mm_err_dev + slot : nullptr;
 }
-static bool mm_take_async_error() {
-  if (g_mm_err_host && *reinterpret_cast<volatile int*>(g_mm_err_host)) { *g_mm_err_host = 0; return true; }
+bool take_async_error(int slot) {
+  if (g_mm_err_host && reinterpret_cast<volatile int*>(g_mm_err_host)[slot]) { g_mm_err_host[slot] = 0; return true; }
   return false;
 }
+int* mm_error_flag_dev() { return async_error_flag_dev(ASYNC_ERR_MATMUL); }
+static bool mm_take_async_error() { return take_async_error(ASYNC_ERR_MATMUL); }
 
 namespace {
 

@@ -107,5 +107,14 @@ dist_neighbor_sample(const at::Tensor& rowptr, const at::Tensor& col, const at::
                  temporal_strategy);
 }
 
+at::Tensor random_walk(const at::Tensor& rowptr, const at::Tensor& col, const at::Tensor& seed, int64_t walk_length, double p,
+                       double q) {
+  const char* fn = "random_walk";   // sampler/random_walk.cpp:15-21
+  require_defined(rowptr, fn, "rowptr"); require_defined(col, fn, "col"); require_defined(seed, fn, "seed");
+  require_same_dtype(rowptr, "rowptr", col, "col", fn); require_same_dtype(rowptr, "rowptr", seed, "seed", fn);
+  static auto op = c10::Dispatcher::singleton().findSchemaOrThrow("pyg::random_walk", "").typed<decltype(random_walk)>();
+  return op.call(rowptr, col, seed, walk_length, p, q);
+}
+
 }  // namespace sampler
 }  // namespace pyg

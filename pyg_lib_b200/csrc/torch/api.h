@@ -58,5 +58,10 @@ dist_neighbor_sample(const at::Tensor& rowptr, const at::Tensor& col, const at::
                      bool csc = false, bool replace = false, bool directed = true, bool disjoint = false,
                      std::string temporal_strategy = "uniform");
 
+// [seed.size(0), walk_length + 1] uniform random walks from `seed` (pyg_lib/csrc/sampler/random_walk.h:10-18); CUDA only,
+// p == q == 1.
+PYGB200_API at::Tensor random_walk(const at::Tensor& rowptr, const at::Tensor& col, const at::Tensor& seed, int64_t walk_length,
+                                   double p = 1.0, double q = 1.0);
+
 }  // namespace sampler
 }  // namespace pyg

@@ -26,7 +26,8 @@ static void cpu_not_supported(const c10::OperatorHandle& op, c10::DispatchKeySet
 
 TORCH_LIBRARY_IMPL(pyg, CPU, m) {   // (the dispatcher has no per-namespace fallback: one registration per CUDA-key op)
   for (const char* name : {"pyg::segment_matmul", "pyg::segment_matmul_bias", "pyg::segment_matmul_wgrad", "pyg::grouped_matmul",
-                           "pyg::neighbor_sample", "pyg::dist_neighbor_sample", "pyg::subgraph", "pyg::relabel_neighborhood"})
+                           "pyg::neighbor_sample", "pyg::dist_neighbor_sample", "pyg::subgraph", "pyg::relabel_neighborhood",
+                           "pyg::random_walk"})
     m.impl(name, torch::CppFunction::makeFromBoxedFunction<&cpu_not_supported>());
 }
 

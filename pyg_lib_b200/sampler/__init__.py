@@ -105,7 +105,7 @@ def hetero_neighbor_sample(
 
 from .dist import dist_neighbor_sample  # noqa: E402  (multi-GPU, frontier-sharded)
 
-__all__ = ['neighbor_sample', 'hetero_neighbor_sample', 'subgraph', 'dist_neighbor_sample']
+__all__ = ['neighbor_sample', 'hetero_neighbor_sample', 'subgraph', 'random_walk', 'dist_neighbor_sample']
 
 
 _subgraph_op = _LazyOp('subgraph')
@@ -122,4 +122,23 @@ def subgraph(
     pointers over :obj:`nodes` (in the given order), target ids relabelled by first occurrence in :obj:`nodes`, and
     (optionally) the positions of the kept edges in :obj:`col`.  CUDA tensors only."""
     return _subgraph_op(rowptr, col, nodes, return_edge_id)
+
+
+_random_walk_op = _LazyOp('random_walk')
+
+
+def random_walk(
+    rowptr: Tensor,
+    col: Tensor,
+    seed: Tensor,
+    walk_length: int,
+    p: float = 1.0,
+    q: float = 1.0,
+) -> Tensor:
+    r"""Samples random walks of length :obj:`walk_length` from all node indices in :obj:`seed` in the graph given by
+    :obj:`(rowptr, col)` — same signature and result as the reference (pyg_lib/sampler/__init__.py:228-254): a tensor
+    of shape :obj:`[seed.size(0), walk_length + 1]` holding the node indices of each walk, equal to the reference's
+    CUDA walker under the same CUDA generator state (and leaving the generator in the same state).  Isolated nodes
+    repeat themselves.  CUDA tensors only; :obj:`p` and :obj:`q` must be 1 (uniform walks), as in the reference."""
+    return _random_walk_op(rowptr, col, seed, walk_length, p, q)
 
