@@ -23,7 +23,7 @@ CXX = '/usr/bin/g++' if osp.exists('/usr/bin/g++') else 'g++'
 CU_SOURCES = ['sampler.cu', 'subgraph.cu', 'matmul.cu', 'matmul_grouped_tc.cu', 'random_walk.cu']
 TORCH_SOURCES = ['torch/library.cpp', 'torch/sampler_op.cpp', 'torch/subgraph_op.cpp', 'torch/matmul_op.cpp', 'torch/api.cpp',
                  'torch/random_walk_op.cpp']
-HEADERS = ['common.cuh', 'mt19937.cuh', 'sampler_v2.cuh', 'sampler_weighted.cuh', 'topk_replay.h', 'mkl_logf_table.inc', 'hopper_ptx.cuh', 'torch/common.h', 'torch/api.h', '../../include/pyg_b200.h']
+HEADERS = ['common.cuh', 'mt19937.cuh', 'sampler_v2.cuh', 'sampler_weighted.cuh', 'topk_replay.h', 'mkl_logf_table.inc', 'hopper_ptx.cuh', 'matmul_common.cuh', 'torch/common.h', 'torch/api.h', '../../include/pyg_b200.h']
 
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '--expt-relaxed-constexpr', '-Xcompiler', '-fPIC', '-ccbin', CXX, '-I' + osp.join(ROOT, 'include'),

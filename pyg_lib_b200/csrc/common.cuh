@@ -75,12 +75,28 @@ struct DevBuf {
   T* as() const { return reinterpret_cast<T*>(p); }
 };
 
-// Stream-ordered scratch that is returned to the pool on every exit path (the PYGB_* macros return early on errors).
+// The stream-ordered allocator's default pool hands memory back to the OS at every synchronisation point, which made
+// matmul run times jump between 2 and 9 ms; keep what it has.
+inline void keep_pool_memory() {
+  static bool done = false;
+  if (done) return;
+  done = true;
+  int dev = 0;
+  cudaMemPool_t pool;
+  if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
+    unsigned long long thr = ~0ull;
+    cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr);
+  }
+}
+
+// Stream-ordered scratch (problem lists, split-K partials) that is returned to the pool on every exit path (the PYGB_*
+// macros return early on errors).
 struct AsyncScratch {
   void* p = nullptr;
   cudaStream_t st = nullptr;
   int alloc(size_t bytes, cudaStream_t stream) {
     st = stream;
+    keep_pool_memory();
     PYGB_CUDA(cudaMallocAsync(&p, bytes, stream));
     return PYGB200_OK;
   }

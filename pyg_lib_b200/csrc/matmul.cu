@@ -6,7 +6,7 @@
 //     `ptr` needs no D2H sync (the reference does size_from_ptr(ptr).cpu(), matmul_kernel.cu:307);
 //   * one launch walks a flat work list over all problems: (128x128 output tile) x (K chunk); ragged
 //     segments load-balance by tiles, and long reductions (the weight gradient dW[b] = X_b^T dY_b, whose
-//     K is the segment length) are split over K chunks that accumulate with fp32 atomics;
+//     K is the segment length) are split over K chunks whose fp32 partials k_finish_split adds in chunk order;
 //   * bf16 / fp16 / fp32 storage with fp32 FMA accumulation; optional fused bias.
 // The tensor-core paths (bf16 / fp16, TF32, and the weight gradient for TMA-aligned shapes) live in
 // matmul_grouped_tc.cu; this file is the path for fp32 ('highest' precision == the reference's SIMT kernels,
@@ -17,7 +17,7 @@
 #include <algorithm>
 #include <vector>
 
-#include "common.cuh"
+#include "matmul_common.cuh"
 
 namespace pygb200 {
 
@@ -56,8 +56,6 @@ bool take_async_error(int slot) {
   if (g_mm_err_host && reinterpret_cast<volatile int*>(g_mm_err_host)[slot]) { g_mm_err_host[slot] = 0; return true; }
   return false;
 }
-int* mm_error_flag_dev() { return async_error_flag_dev(ASYNC_ERR_MATMUL); }
-static bool mm_take_async_error() { return take_async_error(ASYNC_ERR_MATMUL); }
 
 namespace {
 
@@ -89,67 +87,31 @@ __host__ __device__ inline i64 work_items(i64 n, i64 m, i64 k, i64 kchunk) {
   return ceil_div(n, (i64)BM) * ceil_div(m, (i64)BN) * kc;
 }
 
-// problems[b] for segment b of a segment_matmul; also the flat work-item prefix (single block).
+// problems[b] for segment b of a segment_matmul, and the flat work-item prefix (build_segment_list).
 //   mode 0: forward   C_b = X[ptr_b:ptr_b+1] @ W[b]            (n=len, k=K, m=M)
 //   mode 1: wgrad     dW[b] = X_b^T @ dY_b                      (n=K, k=len, m=M), split over K chunks
 __global__ void __launch_bounds__(1024) k_build_segments(Problem* probs, i64* total_tiles, const i64* __restrict__ ptr, const char* x,
                                  const char* w, const char* bias, char* out, float* acc, i64 K, i64 M, i64 B, int esize,
                                  int mode, i64 N, int* err, i64 wgrad_kchunk) {
-  __shared__ i64 s_carry;
-  __shared__ i64 s_w[32];
-  if (threadIdx.x == 0) s_carry = 0;
-  {   // a ptr that is not a segment pointer over [0, N] leaves the launch without work and raises the flag
-    int bad = 0;
-    for (i64 b = threadIdx.x; b < B; b += blockDim.x) bad |= (ptr[b + 1] < ptr[b]) | (b == 0 && ptr[0] != 0) | (b == B - 1 && ptr[B] != N);
-    if (__syncthreads_or(bad)) {
-      if (threadIdx.x == 0) { *total_tiles = 0; if (err) *err = 1; }
-      return;
+  const i64 tiles_mn = ceil_div(K, (i64)BM) * ceil_div(M, (i64)BN);   // wgrad: output tiles of one dW[b]
+  build_segment_list<i64>(probs, total_tiles, ptr, B, N, err, [&](i64 b, i64 r0, i64 len, Problem& p) {
+    if (mode == 0) {
+      p.a = x + r0 * K * esize; p.b = w + b * K * M * esize; p.c = out + r0 * M * esize;
+      p.bias = bias ? bias + b * M * esize : nullptr; p.acc = nullptr;
+      p.n = len; p.k = K; p.m = M; p.sa0 = K; p.sa1 = 1; p.sb0 = M; p.sb1 = 1; p.ldc = M; p.kchunk = K > 0 ? K : 1;
+    } else {
+      p.a = x + r0 * K * esize; p.b = w + r0 * M * esize; p.c = out + b * K * M * esize; p.bias = nullptr;
+      p.n = K; p.k = len; p.m = M; p.sa0 = 1; p.sa1 = K; p.sb0 = M; p.sb1 = 1; p.ldc = M;
+      p.kchunk = wgrad_kchunk;
+      p.acc = (acc != nullptr && len > wgrad_kchunk) ? acc : nullptr;   // (offset past earlier segments' chunks below)
+      if (p.acc == nullptr) p.kchunk = len > 0 ? len : 1;   // short segment: one item, direct store
     }
-  }
-  __syncthreads();
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  for (i64 base = 0; base < B; base += blockDim.x) {
-    const i64 b = base + threadIdx.x;
-    i64 tiles = 0;
-    Problem p;
-    if (b < B) {
-      const i64 r0 = ptr[b], len = ptr[b + 1] - r0;
-      if (mode == 0) {
-        p.a = x + r0 * K * esize; p.b = w + b * K * M * esize; p.c = out + r0 * M * esize;
-        p.bias = bias ? bias + b * M * esize : nullptr; p.acc = nullptr;
-        p.n = len; p.k = K; p.m = M; p.sa0 = K; p.sa1 = 1; p.sb0 = M; p.sb1 = 1; p.ldc = M; p.kchunk = K > 0 ? K : 1;
-      } else {
-        p.a = x + r0 * K * esize; p.b = w + r0 * M * esize; p.c = out + b * K * M * esize; p.bias = nullptr;
-        p.n = K; p.k = len; p.m = M; p.sa0 = 1; p.sa1 = K; p.sb0 = M; p.sb1 = 1; p.ldc = M;
-        p.kchunk = wgrad_kchunk;
-        p.acc = (acc != nullptr && len > wgrad_kchunk) ? acc : nullptr;   // (offset by the chunks before this segment, below)
-        if (p.acc == nullptr) p.kchunk = len > 0 ? len : 1;   // short segment: one item, direct store
-      }
-      tiles = work_items(p.n, p.m, p.k, p.kchunk);
-    }
-    i64 inc = tiles;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const i64 o = __shfl_up_sync(0xffffffffu, inc, d);
-      if (lane >= d) inc += o;
-    }
-    if (lane == 31) s_w[wid] = inc;
-    __syncthreads();
-    i64 pre = 0, tot = 0;
-    for (int q = 0; q < (int)(blockDim.x >> 5); ++q) { if (q < wid) pre += s_w[q]; tot += s_w[q]; }
-    const i64 c0 = s_carry;
-    if (b < B) {
-      p.tile0 = c0 + pre + inc - tiles;
-      // weight gradient: every segment has the same K x M tile grid, so tile0 / (tiles per chunk) numbers the K chunks of
-      // all segments consecutively — chunk c of this segment owns the partial buffer tile0 / tiles_mn + c
-      if (p.acc) p.acc += (p.tile0 / (ceil_div(p.n, (i64)BM) * ceil_div(p.m, (i64)BN))) * p.n * p.m;
-      probs[b] = p;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) s_carry = c0 + tot;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *total_tiles = s_carry;
+    return work_items(p.n, p.m, p.k, p.kchunk);
+  }, [&](Problem& p) {
+    // weight gradient: every segment has the same K x M tile grid, so tile0 / tiles_mn numbers the K chunks of all
+    // segments consecutively — chunk c of this segment owns the partial buffer tile0 / tiles_mn + c
+    if (p.acc) p.acc += (p.tile0 / tiles_mn) * K * M;
+  });
 }
 
 // Generic grouped GEMM.  Work item = (problem, 128x128 output tile, K chunk), taken grid-stride from the
@@ -260,21 +222,12 @@ template <typename T>
 __global__ void k_finish_split(const Problem* __restrict__ probs, i64 P) {
   for (i64 b = blockIdx.y; b < P; b += gridDim.y) {
     const Problem p = probs[b];
-    if (!p.acc) continue;
-    T* C = (T*)p.c;
-    const i64 n = p.n * p.m, chunks = ceil_div(p.k, p.kchunk);
-    for (i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (i64)gridDim.x * blockDim.x) {
-      float v = 0.f;
-      for (i64 c = 0; c < chunks; ++c) v += p.acc[c * n + i];   // fixed order: bit-reproducible
-      C[(i / p.m) * p.ldc + (i % p.m)] = from_f<T>(v);
-    }
+    if (p.acc) finish_split_problem((T*)p.c, p.ldc, p.acc, p.n, p.m, ceil_div(p.k, p.kchunk), [](float v) { return from_f<T>(v); });
   }
 }
 
 int launch_grouped(const Problem* probs_dev, i64 P, const i64* total_dev, i64 tiles_bound, int dtype, cudaStream_t st) {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = num_sms();
   i64 g = tiles_bound < 1 ? 1 : tiles_bound;
   if (g > (i64)sms * 2) g = (i64)sms * 2;   // 2 CTAs of 256 threads x ~128 registers per SM
   void* tk = prof_begin(st);
@@ -291,25 +244,9 @@ int launch_grouped(const Problem* probs_dev, i64 P, const i64* total_dev, i64 ti
 
 inline int esize_of(int dtype) { return dtype == PYGB200_F32 ? 4 : 2; }
 
-// Scratch (problem lists, split-K accumulators) comes from the stream-ordered allocator.  By default that
-// pool hands memory back to the OS at every synchronisation point, which made run times jump between
-// 2 and 9 ms; keep what it has.
-void keep_pool_memory() {
-  static bool done = false;
-  if (done) return;
-  done = true;
-  int dev = 0;
-  cudaMemPool_t pool;
-  if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
-    unsigned long long thr = ~0ull;
-    cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr);
-  }
-}
-
 int segment_generic(const void* x, const i64* ptr_dev, const void* w, const void* bias, void* out, i64 N, i64 K, i64 M,
                     i64 B, int dtype, int mode, cudaStream_t st) {
   if (B == 0) return PYGB200_OK;
-  keep_pool_memory();
   const size_t prob_bytes = (((size_t)B * sizeof(Problem) + 16) + 255) & ~(size_t)255;
   // weight gradient: one fp32 partial [K, M] per K chunk of every split segment (<= N / kchunk + B of them), added up in
   // order afterwards.  The chunk grows until the partials fit 256 MB; if even B of them do not, segments are not split.
@@ -329,7 +266,7 @@ int segment_generic(const void* x, const i64* ptr_dev, const void* w, const void
   i64* total = (i64*)scratch;
   float* acc = split ? (float*)(scratch + prob_bytes) : nullptr;
   k_build_segments<<<1, 1024, 0, st>>>(probs, total, ptr_dev, (const char*)x, (const char*)w, (const char*)bias,
-                                       (char*)out, acc, K, M, B, esize_of(dtype), mode, N, mm_error_flag_dev(), kchunk);
+                                       (char*)out, acc, K, M, B, esize_of(dtype), mode, N, async_error_flag_dev(ASYNC_ERR_MATMUL), kchunk);
   PYGB_LAUNCH_CHECK();
   const i64 bound = mode == 0 ? (ceil_div(N, (i64)BM) + B) * ceil_div(M, (i64)BN)
                               : (ceil_div(N, kchunk) + B) * ceil_div(K, (i64)BM) * ceil_div(M, (i64)BN);
@@ -361,8 +298,8 @@ extern "C" int pygb200_segment_matmul(const void* x, const int64_t* ptr_dev, con
   if (N == 0 || M == 0 || B == 0) return PYGB200_OK;
   PYGB_CHECK(ptr_dev && out && (K == 0 || (x && w)), PYGB200_ERR_ARG, "segment_matmul: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  mm_error_flag_dev();
-  PYGB_CHECK(!mm_take_async_error(), PYGB200_ERR_ARG,
+  async_error_flag_dev(ASYNC_ERR_MATMUL);
+  PYGB_CHECK(!take_async_error(ASYNC_ERR_MATMUL), PYGB200_ERR_ARG,
              "segment_matmul: an EARLIER segment_matmul / wgrad call received an invalid ptr (it must start at 0, be non-decreasing "
              "and end at the number of rows); that call's output is undefined");
   if (K == 0 && bias == nullptr) {
@@ -374,10 +311,8 @@ extern "C" int pygb200_segment_matmul(const void* x, const int64_t* ptr_dev, con
   if (!(flags & PYGB200_MM_FORCE_SIMT) && (flags & PYGB200_MM_ALLOW_TF32) && dtype == PYGB200_F32 &&
       tf32_supported(N, K, M, B, x, w, out))
     return segment_matmul_tf32(x, (const i64*)ptr_dev, w, bias, out, N, K, M, B, st);
-  if (!(flags & PYGB200_MM_FORCE_SIMT) && segment_tc_supported(N, K, M, B, dtype, x, w, out)) {
-    keep_pool_memory();
+  if (!(flags & PYGB200_MM_FORCE_SIMT) && segment_tc_supported(N, K, M, B, dtype, x, w, out))
     return segment_matmul_tc(x, (const i64*)ptr_dev, w, bias, out, N, K, M, B, dtype, st);
-  }
   return segment_generic(x, (const i64*)ptr_dev, w, bias, out, N, K, M, B, dtype, 0, st);
 }
 
@@ -388,10 +323,9 @@ extern "C" int pygb200_segment_matmul_wgrad(const void* x, const int64_t* ptr_de
              "segment_matmul_wgrad: dtype must be f32, bf16 or f16");
   if (K == 0 || M == 0 || B == 0) return PYGB200_OK;
   PYGB_CHECK(ptr_dev && dw && (N == 0 || (x && dy)), PYGB200_ERR_ARG, "segment_matmul_wgrad: null pointer");
-  mm_error_flag_dev();
-  PYGB_CHECK(!mm_take_async_error(), PYGB200_ERR_ARG,
+  async_error_flag_dev(ASYNC_ERR_MATMUL);
+  PYGB_CHECK(!take_async_error(ASYNC_ERR_MATMUL), PYGB200_ERR_ARG,
              "segment_matmul_wgrad: an EARLIER segment_matmul / wgrad call received an invalid ptr; that call's output is undefined");
-  keep_pool_memory();
   if (!(flags & PYGB200_MM_FORCE_SIMT) && N > 0 && wgrad_tc_supported(N, K, M, B, dtype, x, dy, dw))
     return segment_wgrad_tc(x, (const i64*)ptr_dev, dy, dw, N, K, M, B, dtype, (cudaStream_t)stream);
   // empty segments produce zero gradients: their single work item runs the k-loop zero times and stores 0
@@ -404,19 +338,15 @@ extern "C" int pygb200_grouped_matmul(const pygb200_gemm_problem* ps, int64_t co
   PYGB_CHECK(dtype == PYGB200_F32 || dtype == PYGB200_BF16 || dtype == PYGB200_F16, PYGB200_ERR_ARG,
              "grouped_matmul: dtype must be f32, bf16 or f16");
   if (count == 0) return PYGB200_OK;
+  for (i64 i = 0; i < count; ++i) PYGB_CHECK(ps[i].n >= 0 && ps[i].k >= 0 && ps[i].m >= 0, PYGB200_ERR_ARG, "grouped_matmul: negative size");
   cudaStream_t st = (cudaStream_t)stream;
   // bf16 / fp16 problems whose operands satisfy the TMA alignment rules run on the tensor cores (the reference runs
   // grouped_matmul through the same TensorOp grouped GEMM as segment_matmul, matmul_kernel.cu:289-302)
-  if (!(flags & PYGB200_MM_FORCE_SIMT) && grouped_tc_supported(ps, count, dtype)) {
-    for (i64 i = 0; i < count; ++i) PYGB_CHECK(ps[i].n >= 0 && ps[i].k >= 0 && ps[i].m >= 0, PYGB200_ERR_ARG, "grouped_matmul: negative size");
-    keep_pool_memory();
-    return grouped_matmul_tc(ps, count, dtype, st);
-  }
+  if (!(flags & PYGB200_MM_FORCE_SIMT) && grouped_tc_supported(ps, count, dtype)) return grouped_matmul_tc(ps, count, dtype, st);
   std::vector<Problem> h((size_t)count);
   i64 tiles = 0;
   for (i64 i = 0; i < count; ++i) {
     const auto& q = ps[i];
-    PYGB_CHECK(q.n >= 0 && q.k >= 0 && q.m >= 0, PYGB200_ERR_ARG, "grouped_matmul: negative size");
     Problem p;
     p.a = q.a; p.b = q.b; p.c = q.c; p.bias = nullptr; p.acc = nullptr;
     p.n = q.n; p.k = q.k; p.m = q.m;
@@ -429,7 +359,6 @@ extern "C" int pygb200_grouped_matmul(const pygb200_gemm_problem* ps, int64_t co
     h[(size_t)i] = p;
   }
   if (tiles == 0) return PYGB200_OK;
-  keep_pool_memory();
   const size_t bytes = (size_t)count * sizeof(Problem) + 16;
   AsyncScratch sc;
   if (int e = sc.alloc(bytes, st)) return e;

@@ -23,16 +23,14 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
 #include <vector>
 
-#include "common.cuh"
+#include "matmul_common.cuh"
 
 namespace pygb200 {
-int* mm_error_flag_dev();   // matmul.cu
 namespace {
 
 #include "hopper_ptx.cuh"
@@ -49,11 +47,12 @@ constexpr int MAX_SEG = 1024;                              // segments of the TF
 
 // element kinds of the kernel
 constexpr int ET_F16 = 0, ET_BF16 = 1, ET_TF32 = 2;
+inline int et_of(int dtype) { return dtype == PYGB200_BF16 ? ET_BF16 : ET_F16; }   // bf16 / fp16 storage
 
 struct GProb {
   const CUtensorMap* map_a;    // K-major A: dims [k, rows]; MN-major A (transposed view): dims [n, k]
   const CUtensorMap* map_b;    // MN-major B: dims [m, k, z]; K-major B (transposed view): dims [k, m, z]
-  unsigned char* c;            // row-major output of this problem (storage type; fp32 when c_f32)
+  unsigned char* c;            // row-major output of this problem (storage type; fp32 in the TF32 kernel)
   const unsigned char* bias;   // [m] or null (storage type of c)
   i64 ldc;                     // elements
   int n, k, m;
@@ -62,7 +61,6 @@ struct GProb {
   int b_z;                     // third coordinate into map_b (segment index)
   int a_mn, b_k;               // operand stored transposed
   int c_vec;                   // rows of C are 16-byte aligned
-  int c_f32;                   // fp32 output (TF32 kernel)
   int zero_ktail;              // k past `k` in the last stage are rows of the next segment: zero them in shared memory
   int tile0, tiles_n;          // first flat tile of the problem; number of column tiles
   int ksplit, ksteps_chunk;    // K chunks (work items per output tile) and K steps per chunk
@@ -262,7 +260,7 @@ __global__ void __launch_bounds__(GT_NT, 1) k_grouped_wgmma(const GProb* __restr
   }
 }
 
-// segment mode: problems[b] for segment b (all share map_a / map_b), flat tile prefix; one block.
+// segment mode: problems[b] for segment b (all share map_a / map_b), flat tile prefix (build_segment_list).
 //   mode 0 (forward)  C_b = X[ptr_b:ptr_b+1] @ W[b]  (n = len, k = K, m = M); W enters MN-major ([K, M] per segment) or,
 //                      for TF32, K-major ([M, K] per segment, b_k = 1)
 //   mode 1 (wgrad)    dW[b] = X_b^T @ dY_b          (n = K, k = len, m = M): both operands MN-major, every segment split
@@ -270,65 +268,27 @@ __global__ void __launch_bounds__(GT_NT, 1) k_grouped_wgmma(const GProb* __restr
 __global__ void __launch_bounds__(1024) k_gt_build_segments(GProb* probs, int* total, const i64* __restrict__ ptr, const CUtensorMap* map_a,
                                     const CUtensorMap* map_b, unsigned char* out, const unsigned char* bias, int K, int M, int B,
                                     int c_vec, i64 N, int* err, int mode, int esize, int b_k, float* part, int kchunk_steps) {
-  __shared__ int s_carry;
-  __shared__ int s_w[32];
-  if (threadIdx.x == 0) s_carry = 0;
-  {   // a ptr that is not a segment pointer over [0, N] leaves the launch without work and raises the flag
-    int bad = 0;
-    for (int b = threadIdx.x; b < B; b += blockDim.x) bad |= (ptr[b + 1] < ptr[b]) | (b == 0 && ptr[0] != 0) | (b == B - 1 && ptr[B] != N);
-    if (__syncthreads_or(bad)) {
-      if (threadIdx.x == 0) { *total = 0; if (err) *err = 1; }
-      return;
-    }
-  }
-  __syncthreads();
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int tiles_n = (M + GT_BN - 1) / GT_BN, bk = 128 / esize;
   const int tiles_mn = ((K + GT_TM - 1) / GT_TM) * tiles_n;   // wgrad: output tiles of one dW[b]
-  for (int base = 0; base < B; base += blockDim.x) {
-    const int b = base + threadIdx.x;
-    int tiles = 0;
-    GProb p;
-    if (b < B) {
-      const i64 r0 = ptr[b], len = ptr[b + 1] - r0;
-      memset(&p, 0, sizeof(p));
-      p.map_a = map_a; p.map_b = map_b; p.ldc = M; p.m = M; p.a_off = (int)r0; p.tiles_n = tiles_n; p.c_vec = c_vec;
-      if (mode == 0) {
-        p.c = out + r0 * M * esize; p.bias = bias ? bias + (i64)b * M * esize : nullptr;
-        p.n = (int)len; p.k = K; p.b_z = b; p.b_k = b_k; p.c_f32 = esize == 4;
-        p.ksplit = 1; p.ksteps_chunk = (K + bk - 1) / bk;
-        tiles = (int)((len + GT_TM - 1) / GT_TM) * tiles_n;
-      } else {
-        p.c = out + (i64)b * K * M * esize;
-        p.n = K; p.k = (int)len; p.a_mn = 1; p.b_k0 = (int)r0; p.zero_ktail = 1;
-        p.ksteps_chunk = kchunk_steps;
-        p.ksplit = (int)((len + (i64)kchunk_steps * bk - 1) / ((i64)kchunk_steps * bk));
-        tiles = tiles_mn * p.ksplit;
-      }
+  build_segment_list<int>(probs, total, ptr, B, N, err, [&](int b, i64 r0, i64 len, GProb& p) {
+    memset(&p, 0, sizeof(p));
+    p.map_a = map_a; p.map_b = map_b; p.ldc = M; p.m = M; p.a_off = (int)r0; p.tiles_n = tiles_n; p.c_vec = c_vec;
+    if (mode == 0) {
+      p.c = out + r0 * M * esize; p.bias = bias ? bias + (i64)b * M * esize : nullptr;
+      p.n = (int)len; p.k = K; p.b_z = b; p.b_k = b_k;
+      p.ksplit = 1; p.ksteps_chunk = (K + bk - 1) / bk;
+      return (int)((len + GT_TM - 1) / GT_TM) * tiles_n;
     }
-    int inc = tiles;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int o = __shfl_up_sync(0xffffffffu, inc, d);
-      if (lane >= d) inc += o;
-    }
-    if (lane == 31) s_w[wid] = inc;
-    __syncthreads();
-    int pre = 0, tot = 0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { if (w < wid) pre += s_w[w]; tot += s_w[w]; }
-    const int c0 = s_carry;
-    if (b < B) {
-      p.tile0 = c0 + pre + inc - tiles;
-      // wgrad: every segment has the same output tile grid, so tile0 / tiles_mn numbers the K chunks of all segments
-      // consecutively — chunk c of this segment owns partial buffer tile0 / tiles_mn + c
-      if (mode == 1) p.part = part + (i64)(p.tile0 / tiles_mn) * K * M;
-      probs[b] = p;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) s_carry = c0 + tot;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *total = s_carry;
+    p.c = out + (i64)b * K * M * esize;
+    p.n = K; p.k = (int)len; p.a_mn = 1; p.b_k0 = (int)r0; p.zero_ktail = 1;
+    p.ksteps_chunk = kchunk_steps;
+    p.ksplit = (int)((len + (i64)kchunk_steps * bk - 1) / ((i64)kchunk_steps * bk));
+    return tiles_mn * p.ksplit;
+  }, [&](GProb& p) {
+    // wgrad: every segment has the same output tile grid, so tile0 / tiles_mn numbers the K chunks of all segments
+    // consecutively — chunk c of this segment owns partial buffer tile0 / tiles_mn + c
+    if (mode == 1) p.part = part + (i64)(p.tile0 / tiles_mn) * K * M;
+  });
 }
 
 // split-K epilogue: C = sum over the K chunks' partials, in chunk order (bit-reproducible), rounded to the storage type
@@ -336,15 +296,9 @@ template <bool BF16>
 __global__ void k_gt_finish(const GProb* __restrict__ probs, int P) {
   for (int b = blockIdx.y; b < P; b += gridDim.y) {
     const GProb pb = probs[b];
-    if (pb.part == nullptr) continue;
-    const i64 nm = (i64)pb.n * pb.m;
-    for (i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x; i < nm; i += (i64)gridDim.x * blockDim.x) {
-      float v = 0.f;
-      for (int c = 0; c < pb.ksplit; ++c) v += pb.part[(i64)c * nm + i];
-      const i64 r = i / pb.m, col = i - r * pb.m;
-      if (pb.bias) v += ld_bias<BF16>(pb.bias, col);
-      reinterpret_cast<unsigned short*>(pb.c)[r * pb.ldc + col] = (unsigned short)(pack2<BF16>(v, 0.f) & 0xffffu);
-    }
+    if (pb.part)
+      finish_split_problem(reinterpret_cast<unsigned short*>(pb.c), pb.ldc, pb.part, pb.n, pb.m, pb.ksplit,
+                           [](float v) { return (unsigned short)(pack2<BF16>(v, 0.f) & 0xffffu); });
   }
 }
 
@@ -397,13 +351,6 @@ int gt_map(CUtensorMap* m, const void* ptr, int et, int rank, const cuuint64_t* 
 
 constexpr size_t GT_SMEM = 1024 + (size_t)GT_STAGES * GT_STAGE_BYTES + 2 * (size_t)GT_OUT_BYTES + 2 * GT_STAGES * 8;
 
-int num_sms() {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return sms;
-}
-
 template <int ET, int LAYOUT>
 int gt_launch_et(const GProb* probs, int P, const int* total, int grid, cudaStream_t st) {
   PYGB_CUDA(cudaFuncSetAttribute(k_grouped_wgmma<ET, LAYOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GT_SMEM));
@@ -455,7 +402,7 @@ int segment_run(const CUtensorMap (&hm)[2], const i64* ptr_dev, void* out, const
   int* total = reinterpret_cast<int*>(dbuf + total_off);
   k_gt_build_segments<<<1, 1024, 0, st>>>(probs, total, ptr_dev, dm, dm + 1, reinterpret_cast<unsigned char*>(out),
                                           reinterpret_cast<const unsigned char*>(bias), (int)K, (int)M, (int)B, c_vec, N,
-                                          mm_error_flag_dev(), mode, et == ET_TF32 ? 4 : 2, b_k,
+                                          async_error_flag_dev(ASYNC_ERR_MATMUL), mode, et == ET_TF32 ? 4 : 2, b_k,
                                           reinterpret_cast<float*>(dbuf + part_off), kchunk_steps);
   PYGB_LAUNCH_CHECK();
   if (int e = gt_launch(probs, (int)B, total, tiles_bound, et, mode == 0 ? LAY_FWD : LAY_WGRAD, "segment_matmul", st)) return e;
@@ -468,8 +415,7 @@ int segment_run(const CUtensorMap (&hm)[2], const i64* ptr_dev, void* out, const
 // ---- pyg::grouped_matmul: can every problem go through the tensor cores?  (TMA: 16-byte aligned bases and row pitches)
 bool grouped_tc_supported(const pygb200_gemm_problem* ps, i64 count, int dtype) {
   if (dtype != PYGB200_BF16 && dtype != PYGB200_F16) return false;
-  static const bool off = getenv("PYGB200_NO_GROUPED_TC") != nullptr;
-  if (off || count < 1 || count > 65536) return false;
+  if (count < 1 || count > 65536) return false;
   i64 tiles = 0;
   for (i64 i = 0; i < count; ++i) {
     const auto& q = ps[i];
@@ -485,8 +431,7 @@ bool grouped_tc_supported(const pygb200_gemm_problem* ps, i64 count, int dtype) 
 }
 
 int grouped_matmul_tc(const pygb200_gemm_problem* ps, i64 count, int dtype, cudaStream_t st) {
-  const bool bf16 = dtype == PYGB200_BF16;
-  const int et = bf16 ? ET_BF16 : ET_F16;
+  const int et = et_of(dtype);
   const int sms = num_sms();
   // Split-K plan: a weight-gradient-shaped list (few output tiles, very long K: dW = X^T dY of a HeteroDictLinear) would
   // keep a handful of CTAs busy for thousands of K steps.  When the output tiles do not fill the machine twice, every
@@ -567,7 +512,7 @@ int grouped_matmul_tc(const pygb200_gemm_problem* ps, i64 count, int dtype, cuda
     if (cudaMemcpyAsync(dbuf, h.data(), h.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) rc = PYGB200_ERR_CUDA;
     const GProb* dprobs = reinterpret_cast<const GProb*>(dbuf + prob_off);
     if (rc == PYGB200_OK) rc = gt_launch(dprobs, (int)count, reinterpret_cast<const int*>(dbuf + total_off), tiles, et, LAY_ANY, "grouped_gemm", st);
-    if (rc == PYGB200_OK && any_split) rc = finish_launch(dprobs, (int)count, bf16, st);
+    if (rc == PYGB200_OK && any_split) rc = finish_launch(dprobs, (int)count, et == ET_BF16, st);
   }
   return rc;
 }
@@ -575,8 +520,6 @@ int grouped_matmul_tc(const pygb200_gemm_problem* ps, i64 count, int dtype, cuda
 // ---- pyg::segment_matmul, bf16 / fp16
 bool segment_tc_supported(i64 N, i64 K, i64 M, i64 B, int dtype, const void* x, const void* w, const void* out) {
   if (dtype != PYGB200_BF16 && dtype != PYGB200_F16) return false;
-  static const bool off = getenv("PYGB200_NO_GROUPED_TC") != nullptr;
-  if (off) return false;
   if (K < 1 || M < 1 || K % 8 != 0 || M % 8 != 0) return false;
   if (B < 1 || N < 1 || N >= ((i64)1 << 31) || B >= ((i64)1 << 24) || K >= ((i64)1 << 31) || M >= ((i64)1 << 31)) return false;
   if ((N / GT_TM + B) * ((M + GT_BN - 1) / GT_BN) >= ((i64)1 << 31)) return false;
@@ -585,7 +528,7 @@ bool segment_tc_supported(i64 N, i64 K, i64 M, i64 B, int dtype, const void* x, 
 
 int segment_matmul_tc(const void* x, const i64* ptr_dev, const void* w, const void* bias, void* out, i64 N, i64 K, i64 M, i64 B,
                       int dtype, cudaStream_t st) {
-  const int et = dtype == PYGB200_BF16 ? ET_BF16 : ET_F16;
+  const int et = et_of(dtype);
   CUtensorMap hm[2];
   cuuint64_t d[3] = {(cuuint64_t)K, (cuuint64_t)N, 1}, s[2] = {(cuuint64_t)K * 2, 0};
   cuuint32_t box[3] = {64, GT_TM, 1};
@@ -637,7 +580,7 @@ bool wgrad_tc_supported(i64 N, i64 K, i64 M, i64 B, int dtype, const void* x, co
 
 int segment_wgrad_tc(const void* x, const i64* ptr_dev, const void* dy, void* dw, i64 N, i64 K, i64 M, i64 B, int dtype,
                      cudaStream_t st) {
-  const int et = dtype == PYGB200_BF16 ? ET_BF16 : ET_F16;
+  const int et = et_of(dtype);
   CUtensorMap hm[2];
   cuuint64_t d[3] = {(cuuint64_t)K, (cuuint64_t)N, 1}, s[2] = {(cuuint64_t)K * 2, 0};
   cuuint32_t box[3] = {64, 64, 1};   // MN-major A = X^T: box [64 columns of X x 64 rows]

@@ -292,8 +292,9 @@ def test_segment_forward_tf32_exact(lib, K, M):
 
 @gpu
 def test_segment_forward_many_segments_exact(lib):
-    """B = 3000 segments, most of them empty or 1 row and a few long: the multi-pass prefix loops of k_gt_build_segments
-    (bf16, tensor cores) and k_build_segments (fp32 with TF32 allowed, which takes SIMT because B > 1024)."""
+    """B = 3000 segments, most of them empty or 1 row and a few long: the multi-pass prefix loop of build_segment_list,
+    through the tensor-core builder k_gt_build_segments (bf16) and the SIMT builder k_build_segments (fp32 with TF32
+    allowed, which takes SIMT because B > 1024)."""
     g = torch.Generator().manual_seed(3000)
     lens = torch.randint(0, 2, (3000,), generator=g)
     lens[[5, 1023, 1024, 2047, 2999]] = torch.tensor([700, 300, 129, 64, 1000])
@@ -318,8 +319,9 @@ WGRAD_LENS = [0, 1, 63, 65, 100, 0, 2100, 5000, 130, 4099]
 @pytest.mark.parametrize('dtype', LOWP)
 @pytest.mark.parametrize('M', [64, 192, 256])
 def test_wgrad_tensor_cores_exact(lib, abi, dtype, M):
-    """k_grouped_wgmma<LAY_WGRAD> (zero_ktail) + k_gt_finish: lengths not multiples of 64, segments of several 2048-row
-    chunks, empty segments (zeros); and the same data through the SIMT split path (FORCE_SIMT, k_finish_split)."""
+    """k_grouped_wgmma<LAY_WGRAD> (zero_ktail) + k_gt_finish (finish_split_problem, pack2): lengths not multiples of 64,
+    segments of several 2048-row chunks, empty segments (zeros); and the same data through the SIMT split path
+    (FORCE_SIMT, k_finish_split: finish_split_problem, from_f)."""
     K = 128
     g = torch.Generator().manual_seed(M)
     ptr = ragged(WGRAD_LENS)
@@ -338,7 +340,8 @@ def test_wgrad_tensor_cores_exact(lib, abi, dtype, M):
 @pytest.mark.parametrize('case', ['off_shape', 'b1025'])
 def test_wgrad_simt_split_exact(lib, dtype, case):
     """the SIMT weight gradient through the op: K / M off the tensor-core shapes, and B = 1025 (> MAX_SEG of the
-    tensor-core path) — lengths > 2048 so that k_finish_split<T> runs, in fp16 as well as bf16"""
+    tensor-core path) — lengths > 2048 so that k_finish_split<T> (finish_split_problem with from_f) runs, in fp16 as
+    well as bf16"""
     g = torch.Generator().manual_seed(1025 if case == 'b1025' else 96)
     if case == 'off_shape':
         K, M, lens = 96, 72, WGRAD_LENS
@@ -400,7 +403,8 @@ def test_grouped_layouts_exact(lib, abi, dtype, a_t, b_t):
 @gpu
 @pytest.mark.parametrize('dtype', LOWP)
 def test_grouped_split_k_exact(lib, dtype):
-    """one [128 x 65536] @ [65536 x 128] problem: few output tiles, long K -> grouped split-K + k_gt_finish"""
+    """one [128 x 65536] @ [65536 x 128] problem: few output tiles, long K -> grouped split-K + k_gt_finish
+    (finish_split_problem, pack2)"""
     g = torch.Generator().manual_seed(65536)
     a, b = int_tensor(g, (128, 65536), 6), int_tensor(g, (65536, 128), 6)
     exp = to_storage(exact_mm(a, b), dtype)
@@ -540,7 +544,8 @@ TIE_SITES = ['tc_vector', 'tc_tail', 'tc_split_wgrad', 'tc_split_grouped', 'simt
 @pytest.mark.parametrize('site', TIE_SITES)
 def test_rounding_ties(lib, abi, dtype, site):
     """the fixed tie table through each fp32 -> storage conversion: tensor-core vector store (pack2), tensor-core scalar
-    tail store, k_gt_finish after a weight gradient and after a grouped split-K, SIMT from_f, k_finish_split"""
+    tail store, k_gt_finish (pack2) after a weight gradient and after a grouped split-K, SIMT from_f, k_finish_split
+    (from_f); the two finishers share the chunk-sum loop finish_split_problem"""
     if site in ('tc_vector', 'simt'):
         A, Bm, exp = tie_operands(dtype, 16, 64, 136)
         x, w = A.to(dtype).to(DEV), Bm.to(dtype).to(DEV)[None]

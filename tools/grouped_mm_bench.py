@@ -1,5 +1,5 @@
 """grouped_matmul / general-shape segment_matmul on the tensor cores (matmul_grouped_tc.cu): time, TFLOP/s and the
-fraction of each shape's roofline (min of the measured HBM and bf16 peaks), next to the SIMT path (PYGB200_NO_GROUPED_TC).
+fraction of each shape's roofline (min of the measured HBM and bf16 peaks).
 
     python tools/grouped_mm_bench.py > gpurun_out/grouped_mm.json
 
@@ -7,7 +7,6 @@ Shapes: HeteroDictLinear-like problem lists (VERDICT r1 item 4: 8 x [100k,256]@[
 specialised segment kernel does not take (32, 96, 512, 1024), and the backward views (dX, dW)."""
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -45,7 +44,7 @@ def main():
                     bound='hbm' if byts / (peaks['hbm_gbs'] * 1e9) > flops / (peaks['bf16_tflops'] * 1e12) else 'tensor')
 
     g = torch.Generator().manual_seed(0)
-    res = {'tc_enabled': os.environ.get('PYGB200_NO_GROUPED_TC') is None, 'grouped': {}, 'segment': {}}
+    res = {'grouped': {}, 'segment': {}}
     for name, shapes in (('8x[100k,256]@[256,256]', [(100_000, 256, 256)] * 8),
                          ('8x[100k,128]@[128,128]', [(100_000, 128, 128)] * 8),
                          ('ragged 16 relations 64->64', [(int(n), 64, 64) for n in (ragged_ptr(1 << 20, 16, 7)[1:] - ragged_ptr(1 << 20, 16, 7)[:-1])]),
@@ -74,12 +73,4 @@ def main():
 
 
 if __name__ == '__main__':
-    if '--child' in sys.argv:
-        print('GMM ' + json.dumps(main()))
-    else:
-        out = {}
-        for label, env in (('tensor_cores', {}), ('simt', {'PYGB200_NO_GROUPED_TC': '1'})):
-            r = subprocess.run([sys.executable, os.path.abspath(__file__), '--child'], env=dict(os.environ, **env), capture_output=True, text=True)
-            line = [ln for ln in r.stdout.splitlines() if ln.startswith('GMM ')]
-            out[label] = json.loads(line[0][4:]) if line else {'error': r.stderr[-1500:]}
-        print(json.dumps(out))
+    print(json.dumps(main()))
