@@ -10,12 +10,18 @@
 // sample_node (draws: Robert Floyd / with replacement / full row; coalesced writes of (row, global dst, edge id);
 // hash insert keyed by global id with a min-reduction of the flat emission position = first-occurrence order),
 // mark_tile (an edge is "first" iff its position won the reduction; tile-local ranks).
-//   latency path     k_seed_fused (+ the first pass's count) -> per pass k_count_s, k_sample_s, k_mark_s, k_assign_s
-//                    -> k_final: write-once counters, every block scans the <= 1024 tile aggregates itself, the run is
-//                    published to the host by its last pass (DESIGN.md 3.3).  Small bounded runs.
-//   throughput path  k_seed* -> per pass k_count, k_sample, k_mark, k_assign (last block scans, running counters)
-//                    -> k_final: any size, full neighbourhoods (host-synced sizing), frontier sharding, no-dedup hop.
-// Host work per call: bounds, launches, ONE wait on a mapped flag (the API returns host counts).
+// Three schedules:
+//   latency      k_seed_fused (+ the first pass's count) -> per pass k_count_s, k_sample_s, k_mark_s, k_assign_s
+//                -> k_final: write-once counters, every block scans the <= 1024 tile aggregates itself, the run is
+//                published to the host by its last pass (DESIGN.md 3.3).  Small bounded runs.
+//   v2           (sampler_v2.cuh) k_v2_seed -> per pass k_count, k_v2_sample (+ inserts), k_v2_mark, k_v2_assign -> k_final:
+//                packed 32-bit table, refs instead of lookups, peer-memory frontier sharding.  The other bounded,
+//                non-disjoint runs whose node ids fit 32 bits.
+//   wide table   k_seed* -> per pass k_count, k_sample, k_mark, k_assign (last block scans, running counters)
+//                -> k_final: any size, full neighbourhoods (host-synced sizing), disjoint / temporal runs, collective
+//                frontier sharding, no-dedup hop.
+// Host work per call: bounds, launches, ONE wait on a mapped flag (the API returns host counts).  make_plan decides
+// everything about a run before its first CUDA call; Run<idx_t> executes it phase by phase.
 #include <dlfcn.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -1446,6 +1452,32 @@ extern "C" void pygb200_sampler_destroy(pygb200_sampler* s) {
 
 namespace {
 
+// kernel<<<grid, block, smem, st>>>(args...), as a PDL launch (with the programmatic-stream-serialization attribute, see
+// pdl_enter) or a plain one, timed under the profile slot `slot` with `work` units (no slot: not timed).  Counts the
+// launch and returns its error.
+constexpr bool PDL = true, PLAIN = false;
+template <bool pdl, typename... KP, typename... A>
+int launch(const char* slot, long long work, void (*kernel)(KP...), dim3 grid, int block, size_t smem, cudaStream_t st,
+           A... args) {
+  void* tk = slot ? prof_begin(st) : nullptr;
+  cudaError_t err = cudaSuccess;
+  if constexpr (pdl) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid; cfg.blockDim = dim3((unsigned)block); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    err = cudaLaunchKernelEx(&cfg, kernel, KP(args)...);
+  } else {
+    kernel<<<grid, block, smem, st>>>(KP(args)...);
+  }
+  prof_end(tk, slot, st, work);
+  PYGB_CUDA(err);
+  PYGB_LAUNCH_CHECK();
+  return PYGB200_OK;
+}
+
 constexpr int MAX_SHARDS = 64;
 struct Layout { int o_list, o_ids, o_begin, o_end, o_rel, o_nph, o_eph, o_mt, o_shard, o_ssa; size_t words; };
 Layout make_layout(int T, int R, int L) {
@@ -1487,9 +1519,9 @@ int ensure_table(pygb200_sampler* s, int t, i64 need_nodes, i64 listed, cudaStre
     if (int e = nv.ensure(cap * 8, 0, st)) return e;
     PYGB_CUDA(cudaMemsetAsync(nk.p, 0xff, nk.cap, st));
     PYGB_CUDA(cudaMemsetAsync(nv.p, 0xff, nv.cap, st));
-    k_rehash<<<grid_for(listed, NT, s->sm_count), NT, 0, st>>>(tb.keys.as<u64>(), tb.vals.as<u64>(), nk.as<u64>(),
-                                                              nv.as<u64>(), cap - 1, tb.slot.as<u32>(), listed);
-    PYGB_LAUNCH_CHECK();
+    if (int e = launch<PLAIN>(nullptr, 0, k_rehash, grid_for(listed, NT, s->sm_count), NT, 0, st, tb.keys.as<u64>(), tb.vals.as<u64>(),
+                              nk.as<u64>(), nv.as<u64>(), cap - 1, tb.slot.as<u32>(), listed))
+      return e;
     PYGB_CUDA(cudaStreamSynchronize(st));
     tb.keys.release(); tb.vals.release();
     tb.keys = nk; tb.vals = nv;
@@ -1584,18 +1616,6 @@ int ensure_edge_scratch(pygb200_sampler* s, i64 E, cudaStream_t st) {
   return PYGB200_OK;
 }
 
-// kernel<<<grid, block, smem, st>>>(args...) with the programmatic-stream-serialization attribute (see pdl_enter)
-template <typename... KP, typename... A>
-cudaError_t launch_pdl(void (*kernel)(KP...), dim3 grid, int block, size_t smem, cudaStream_t st, A... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid; cfg.blockDim = dim3((unsigned)block); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kernel, KP(args)...);
-}
-
 // jump-ahead table: mt19937_jump.bin next to this shared library (optional; without it generation is serial)
 void load_jump_table(pygb200_sampler* s, cudaStream_t st) {
   if (s->jump_tried) return;
@@ -1642,83 +1662,103 @@ int mt_request(pygb200_sampler* s, cudaStream_t st, i64 target) {
     if (s->jump_P >= 2 && amount >= std::max<i64>(2 * (i64)s->jump_S, JUMP_MIN_WORDS)) {
       const int P_used = (int)std::min<i64>(s->jump_P, (amount + s->jump_S - 1) / s->jump_S);
       i64* jb = s->jump_scratch.as<i64>();
-      k_mt_jump_prestep<3><<<1, 640, 0, st>>>(s->raw.as<u32>(), s->gen.as<i64>(), jb, s->raw_cap_words);
-      PYGB_LAUNCH_CHECK();
+      if (int e = launch<PLAIN>(nullptr, 0, k_mt_jump_prestep<3>, 1, 640, 0, st, s->raw.as<u32>(), s->gen.as<i64>(), jb, s->raw_cap_words))
+        return e;
       static const bool smem_ok = cudaFuncSetAttribute(k_mt_jump_generate<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, MT_JUMP_HIST * 4) == cudaSuccess;
       PYGB_CHECK(smem_ok, PYGB200_ERR_CUDA, "k_mt_jump_generate: cannot reserve shared memory for the jump history");
-      k_mt_jump_generate<3><<<P_used, 640, MT_JUMP_HIST * 4, st>>>(s->raw.as<u32>(), s->gen.as<i64>(), jb, s->jump_polys.as<u32>(), s->jump_S,
-                                                                  s->raw_cap_words, reinterpret_cast<unsigned long long*>(jb + 1));
-      PYGB_LAUNCH_CHECK();
+      if (int e = launch<PLAIN>(nullptr, 0, k_mt_jump_generate<3>, P_used, 640, MT_JUMP_HIST * 4, st, s->raw.as<u32>(), s->gen.as<i64>(), jb,
+                                s->jump_polys.as<u32>(), s->jump_S, s->raw_cap_words, reinterpret_cast<unsigned long long*>(jb + 1)))
+        return e;
       s->mt_requested += (i64)P_used * s->jump_S;
       if (s->mt_requested > s->raw_cap_words - MT_N) { s->mt_requested = s->raw_cap_words - MT_N; break; }
     } else {
-      k_mt_extend_to<3><<<1, 640, 0, st>>>(s->raw.as<u32>(), s->gen.as<i64>(), target, s->raw_cap_words);
-      PYGB_LAUNCH_CHECK();
+      if (int e = launch<PLAIN>(nullptr, 0, k_mt_extend_to<3>, 1, 640, 0, st, s->raw.as<u32>(), s->gen.as<i64>(), target, s->raw_cap_words))
+        return e;
       s->mt_requested = target;
     }
   }
   return PYGB200_OK;
 }
 
-template <typename idx_t>
-int launch_count(pygb200_sampler* s, const PassArgs& a, i64 F, i64 E_prev, cudaStream_t st) {
-  // the grid also has to cover the deferred lookup of the previous pass (E_prev edges)
-  const int g = std::max(grid_for(F, NT, s->sm_count), a.lk_colv ? grid_for(E_prev, NT, s->sm_count) : 1);
-  void* tk = prof_begin(st);
-  launch_pdl(k_count<idx_t>, g, NT, 0, st, a);
-  prof_end(tk, "count", st, F);
-  PYGB_LAUNCH_CHECK();
+int biased_error(i64 code) {
+  PYGB_CHECK(code != W_ERR_NEG, PYGB200_ERR_ARG, "invalid multinomial distribution (encountering probability entry < 0)");
+  PYGB_CHECK(code != W_ERR_INF, PYGB200_ERR_ARG, "invalid multinomial distribution (encountering probability entry = infinity or NaN)");
+  PYGB_CHECK(code != W_ERR_SUM, PYGB200_ERR_ARG, "invalid multinomial distribution (sum of probabilities <= 0)");
+  PYGB_CHECK(code != W_ERR_CATEGORIES, PYGB200_ERR_ARG, "number of categories cannot exceed 2^24");
   return PYGB200_OK;
 }
 
-template <typename idx_t>
-int launch_sample(pygb200_sampler* s, const PassArgs& a_in, i64 F, i64 E, cudaStream_t st) {
-  PassArgs a = a_in;
-  a.group = sample_group_lanes(a.fanout);
-  const int gs = grid_for(F, sample_nodes_per_block(a.group), s->sm_count);
-  void* tk = prof_begin(st);
-  launch_pdl(k_sample<idx_t>, gs, NT, 0, st, a);
-  prof_end(tk, "sample", st, E);
-  PYGB_LAUNCH_CHECK();
-  return PYGB200_OK;
+u64 xbar_timeout_ns() {
+  static const u64 ns = [] { const char* e = getenv("PYGB200_XBARRIER_TIMEOUT_MS"); return (u64)(e ? atoll(e) : 20000) * 1000000ull; }();
+  return ns;
 }
 
-template <typename idx_t>
-int launch_rest(pygb200_sampler* s, const PassArgs& a, i64 F, i64 E, bool lookup_now, cudaStream_t st, bool with_sample = true) {
-  if (with_sample) if (int e = launch_sample<idx_t>(s, a, F, E, st)) return e;
-  void* tk = prof_begin(st);
-  launch_pdl(k_mark, grid_for(E, ETILE, s->sm_count), NT, 0, st, a);
-  prof_end(tk, "mark", st, E);
-  PYGB_LAUNCH_CHECK();
-  tk = prof_begin(st);
-  launch_pdl(k_assign, grid_for(E, NT, s->sm_count), NT, 0, st, a);
-  prof_end(tk, "assign", st, E);
-  PYGB_LAUNCH_CHECK();
-  if (lookup_now) {
-    tk = prof_begin(st);
-    k_lookup<<<grid_for(E, NT, s->sm_count), NT, 0, st>>>(a);
-    prof_end(tk, "lookup", st, E);
-    PYGB_LAUNCH_CHECK();
-  }
-  return PYGB200_OK;
+// ------------------------------------------------------------------------------------- run plan
+// Static worst case of a run: frontier per (type, hop) `fb` and edges per (relation, hop) `eb` (every frontier node emits
+// <= k edges, every edge adds <= one node of the relation's dst type; a fan-out < 0 adds nothing), and their sums per type
+// (`nodes`) and per relation (`edges`).  Unclamped; every sum saturates at 2^60.  The relations' endpoints must be valid.
+void static_bounds(int T, int R, int L, const pygb200_relation* rels, const int64_t* n_seeds, const int64_t* num_neighbors,
+                   std::vector<i64>& fb, std::vector<i64>& eb, std::vector<i64>& nodes, std::vector<i64>& edges) {
+  fb.assign((size_t)T * (L + 1), 0);
+  eb.assign((size_t)R * (L > 0 ? L : 1), 0);
+  for (int t = 0; t < T; ++t) fb[(size_t)t * (L + 1)] = n_seeds[t];
+  for (int h = 0; h < L; ++h)
+    for (int r = 0; r < R; ++r) {
+      const i64 k = num_neighbors[(size_t)r * L + h];
+      const i64 e = k >= 0 ? sat_mul(fb[(size_t)rels[r].src_type * (L + 1) + h], k) : 0;
+      eb[(size_t)r * L + h] = e;
+      i64& nf = fb[(size_t)rels[r].dst_type * (L + 1) + h + 1];
+      nf = sat_add(nf, e);
+    }
+  nodes.assign(T, 0);
+  edges.assign(R, 0);
+  for (int t = 0; t < T; ++t)
+    for (int h = 0; h <= L; ++h) nodes[t] = sat_add(nodes[t], fb[(size_t)t * (L + 1) + h]);
+  for (int r = 0; r < R; ++r)
+    for (int h = 0; h < L; ++h) edges[r] = sat_add(edges[r], eb[(size_t)r * L + h]);
 }
 
-int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const pygb200_relation* rels,
-                     const void* const* seeds, const int64_t* n_seeds, const int64_t* num_neighbors,
-                     unsigned flags, pygb200_mt19937* mt, int64_t* nodes_per_hop, int64_t* edges_per_hop,
-                     int64_t* n_nodes_out, int64_t* n_edges_out, cudaStream_t st, const pygb200_shard* shard,
-                     const pygb200_temporal* temporal, const void* const* edge_weight = nullptr) {
-  const bool replace = flags & PYGB200_S_REPLACE, disjoint = flags & PYGB200_S_DISJOINT, idx32 = flags & PYGB200_S_INDEX32;
-  // the output binding is one-shot: it is consumed here, before any check can return early, so that a failed run
-  // never leaves pointers to arrays its caller is about to free (ADVICE r1)
-  const bool bound_armed = s->bound.armed;
-  s->bound.armed = false;
-  s->last_direct = false;
+// Everything a run decides before its first CUDA call: the caller's arguments, the static bounds, the mode flags and the
+// schedule.
+struct RunPlan {
+  int T = 0, R = 0, L = 0;
+  const pygb200_relation* rels = nullptr;
+  const void *const *seeds = nullptr, *const *edge_weight = nullptr;
+  const int64_t *n_seeds = nullptr, *num_neighbors = nullptr;
+  unsigned flags = 0;
+  const pygb200_shard* shard = nullptr;
+  const pygb200_temporal* temporal = nullptr;
+  bool replace = false, disjoint = false, idx32 = false;
   i64 total_seeds = 0;
+  std::vector<i64> fb, eb, node_cap, rel_cap;   // static_bounds; the capacities clamped to >= 1
+  i64 max_F = 1, max_E = 1, draw_units = 0, draw_count = 0;
+  bool synced = false;   // sync after every count kernel and size buffers from actual numbers
+  bool any_time = false, weighted = false, mixed = false, sharded = false, p2p = false, nodedup = false;
+  std::vector<char> wrel;          // relations with edge weights
+  std::vector<i64> type_nodes;     // nodes of each type, where a relation with that source type tells us (-1: unknown)
+  bool lat = false, v2 = false;    // the schedule: latency, v2, else the wide table
+  bool direct = false;             // results straight into the caller's bound arrays
+  int XW = 1, XR = 0;              // peer-memory sharding: world size and rank
+  int fuse_r = -1, fuse_t = -1;    // latency schedule: the first pass, counted inside the seed launch of its source type
+  i64 k(int r, int h) const { return num_neighbors[(size_t)r * L + h]; }
+  i64 F(int r, int h) const { return fb[(size_t)rels[r].src_type * (L + 1) + h]; }   // static frontier of pass (h, r)
+  i64 E(int r, int h) const { return eb[(size_t)r * L + h]; }
+  bool launches(int r, int h) const { return k(r, h) != 0 && F(r, h) != 0 && E(r, h) != 0; }   // bounded pass (h, r) runs
+};
+
+int make_plan(RunPlan& p, pygb200_sampler* s, bool bound_armed, int32_t T, int32_t R, int32_t L, const pygb200_relation* rels,
+              const void* const* seeds, const int64_t* n_seeds, const int64_t* num_neighbors, unsigned flags,
+              const pygb200_mt19937* mt, const pygb200_shard* shard, const pygb200_temporal* temporal,
+              const void* const* edge_weight) {
+  p.T = T; p.R = R; p.L = L; p.rels = rels; p.seeds = seeds; p.n_seeds = n_seeds; p.num_neighbors = num_neighbors;
+  p.flags = flags; p.shard = shard; p.temporal = temporal; p.edge_weight = edge_weight;
+  const bool replace = p.replace = (flags & PYGB200_S_REPLACE) != 0;
+  const bool disjoint = p.disjoint = (flags & PYGB200_S_DISJOINT) != 0;
+  const bool idx32 = p.idx32 = (flags & PYGB200_S_INDEX32) != 0;
   for (int t = 0; t < T; ++t) {
     PYGB_CHECK(n_seeds[t] >= 0, PYGB200_ERR_ARG, "negative seed count");
     PYGB_CHECK(n_seeds[t] == 0 || seeds[t] != nullptr, PYGB200_ERR_ARG, "null seed pointer");
-    total_seeds += n_seeds[t];
+    p.total_seeds += n_seeds[t];
   }
   for (int r = 0; r < R; ++r) {
     PYGB_CHECK(rels[r].src_type >= 0 && rels[r].src_type < T && rels[r].dst_type >= 0 && rels[r].dst_type < T,
@@ -1728,48 +1768,35 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
     PYGB_CHECK(rels[r].rowptr != nullptr && (rels[r].col != nullptr || rels[r].num_edges == 0), PYGB200_ERR_ARG,
                "null CSR pointer");
   }
-  if (disjoint) PYGB_CHECK(total_seeds < ((i64)1 << 23), PYGB200_ERR_UNSUPPORTED,
+  if (disjoint) PYGB_CHECK(p.total_seeds < ((i64)1 << 23), PYGB200_ERR_UNSUPPORTED,
                            "disjoint sampling supports < 2^23 seeds and node ids < 2^40 on this path");
   PYGB_CHECK(mt->left >= 1 && mt->left <= MT_N && mt->next >= 0 && mt->next <= MT_N, PYGB200_ERR_ARG,
              "invalid mt19937 state");
 
-  // ---- static worst-case bounds: frontier per (type, hop), edges per (relation, hop)
-  const int Lz = L > 0 ? L : 1;
-  std::vector<i64> fb((size_t)T * (L + 1), 0), eb((size_t)R * Lz, 0);
-  for (int t = 0; t < T; ++t) fb[(size_t)t * (L + 1)] = n_seeds[t];
-  bool synced = false;  // true: sync after every count kernel and size buffers from actual numbers
-  for (int h = 0; h < L; ++h)
-    for (int r = 0; r < R; ++r) {
-      const i64 k = num_neighbors[(size_t)r * L + h];
-      const i64 F = fb[(size_t)rels[r].src_type * (L + 1) + h];
-      if (k < 0) synced = true;
-      const i64 e = k >= 0 ? sat_mul(F, k) : 0;
-      eb[(size_t)r * L + h] = e;
-      i64& nf = fb[(size_t)rels[r].dst_type * (L + 1) + h + 1];
-      nf = sat_add(nf, e);
-    }
-  std::vector<i64> node_cap(T, 0), rel_cap(R, 0);
-  i64 max_F = 1, max_E = std::max<i64>(total_seeds, 1), draw_units = 0, draw_count = 0, total_elems = 0;
+  // ---- static worst-case bounds
+  static_bounds(T, R, L, rels, n_seeds, num_neighbors, p.fb, p.eb, p.node_cap, p.rel_cap);
+  bool& synced = p.synced;
+  for (size_t i = 0; i < (size_t)R * L; ++i) if (num_neighbors[i] < 0) synced = true;   // full neighbourhoods: no bound
+  i64 total_elems = 0;
+  p.max_E = std::max<i64>(p.total_seeds, 1);
   for (int t = 0; t < T; ++t) {
-    i64 c = 0;
-    for (int h = 0; h <= L; ++h) { c = sat_add(c, fb[(size_t)t * (L + 1) + h]); max_F = std::max(max_F, fb[(size_t)t * (L + 1) + h]); }
-    node_cap[t] = std::max<i64>(c, 1);
-    total_elems = sat_add(total_elems, c);
+    for (int h = 0; h <= L; ++h) p.max_F = std::max(p.max_F, p.fb[(size_t)t * (L + 1) + h]);
+    total_elems = sat_add(total_elems, p.node_cap[t]);
+    p.node_cap[t] = std::max<i64>(p.node_cap[t], 1);
   }
   for (int r = 0; r < R; ++r) {
-    i64 c = 0;
     for (int h = 0; h < L; ++h) {
-      const i64 e = eb[(size_t)r * L + h];
-      c = sat_add(c, e); max_E = std::max(max_E, e);
+      const i64 e = p.E(r, h);
+      p.max_E = std::max(p.max_E, e);
       // units per draw: 1 when every range < 2^16, else at most 2 + 1 skipped (32-bit) / 4 + 3 (64-bit)
-      draw_units = sat_add(draw_units, sat_mul(e, rels[r].num_edges < 65536 ? 1 : (rels[r].num_edges < ((i64)1 << 32) ? 3 : 7)));
-      draw_count = sat_add(draw_count, e);
+      p.draw_units = sat_add(p.draw_units, sat_mul(e, rels[r].num_edges < 65536 ? 1 : (rels[r].num_edges < ((i64)1 << 32) ? 3 : 7)));
+      p.draw_count = sat_add(p.draw_count, e);
     }
-    rel_cap[r] = std::max<i64>(c, 1);
-    total_elems = sat_add(total_elems, sat_mul(c, 3));
+    total_elems = sat_add(total_elems, sat_mul(p.rel_cap[r], 3));
+    p.rel_cap[r] = std::max<i64>(p.rel_cap[r], 1);
   }
   if (total_elems > ((i64)1 << 30)) synced = true;  // > 8 GiB of worst-case int64 results: size from actuals
-  bool any_time = false;
+  bool& any_time = p.any_time;
   if (temporal) {
     for (int t = 0; t < T && temporal->node_time; ++t) any_time |= temporal->node_time[t] != nullptr;
     for (int r = 0; r < R && temporal->edge_time; ++r) any_time |= temporal->edge_time[r] != nullptr;
@@ -1782,25 +1809,24 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
   }
   // biased sampling (edge_weight): per relation (neighbor_kernel.cpp:732-745).  `mixed` = some relations with weights, some without:
   // the weighted ones take engine outputs directly while the others draw from the RandintEngine, whose 256-output blocks then sit
-  // wherever the generator happened to be when a block ran out — see "mixed" below.
-  bool weighted = false, mixed = false;
-  std::vector<char> wrel((size_t)std::max(R, 1), 0);
+  // wherever the generator happened to be when a block ran out — see Run::hops_synced.
+  p.wrel.assign((size_t)std::max(R, 1), 0);
   if (edge_weight) {
     int nw = 0;
-    for (int r = 0; r < R; ++r) { wrel[r] = edge_weight[r] != nullptr; nw += wrel[r]; }
-    weighted = nw > 0;
-    mixed = nw > 0 && nw < R;
-    PYGB_CHECK(!weighted || !any_time, PYGB200_ERR_ARG, "Biased temporal sampling not yet supported");   // neighbor_kernel.cpp:377-380
-    if (weighted && replace)
+    for (int r = 0; r < R; ++r) { p.wrel[r] = edge_weight[r] != nullptr; nw += p.wrel[r]; }
+    p.weighted = nw > 0;
+    p.mixed = nw > 0 && nw < R;
+    PYGB_CHECK(!p.weighted || !any_time, PYGB200_ERR_ARG, "Biased temporal sampling not yet supported");   // neighbor_kernel.cpp:377-380
+    if (p.weighted && replace)
       for (int r = 0; r < R; ++r)
-        for (int h = 0; h < L && wrel[r]; ++h)
-          PYGB_CHECK(num_neighbors[(size_t)r * L + h] != 1, PYGB200_ERR_UNSUPPORTED,
+        for (int h = 0; h < L && p.wrel[r]; ++h)
+          PYGB_CHECK(p.k(r, h) != 1, PYGB200_ERR_UNSUPPORTED,
                      "biased sampling with replacement and a fan-out of 1: at::multinomial(n_sample=1) draws from an MKL VSL stream "
                      "(exponential_), which this path does not reproduce");
   }
-  if (mixed) synced = true;   // the host follows the engine's block count pass by pass
-  const bool sharded = shard != nullptr && shard->world > 1;
-  const bool nodedup = (flags & PYGB200_S_NO_DEDUP) != 0;
+  if (p.mixed) synced = true;   // the host follows the engine's block count pass by pass
+  const bool sharded = p.sharded = shard != nullptr && shard->world > 1;
+  const bool nodedup = p.nodedup = (flags & PYGB200_S_NO_DEDUP) != 0;
   if (nodedup) PYGB_CHECK(T == 1 && R == 1 && L == 1 && !sharded, PYGB200_ERR_ARG,
                           "PYGB200_S_NO_DEDUP (distributed one-hop sampling) takes one node type, one relation, one hop");
   s->last_nodedup = false;
@@ -1814,114 +1840,156 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
   // ids provably fit 32 bits, the wide-table throughput path for everything else.
   static const bool no_lat = getenv("PYGB200_NO_LATENCY_PATH") != nullptr;
   static const bool no_v2 = getenv("PYGB200_NO_V2") != nullptr;
-  bool lat = !synced && !sharded && !nodedup && L > 0 && !no_lat && !weighted;
+  bool& lat = p.lat;
+  lat = !synced && !sharded && !nodedup && L > 0 && !no_lat && !p.weighted;
   for (int t = 0; t < T && lat; ++t) lat = n_seeds[t] <= SEED_FUSED_MAX;
   for (int h = 0; h < L && lat; ++h)
     for (int r = 0; r < R && lat; ++r) {
-      if (num_neighbors[(size_t)r * L + h] == 0) continue;
-      lat = fb[(size_t)rels[r].src_type * (L + 1) + h] <= (i64)LAT_TILES * NT && eb[(size_t)r * L + h] <= (i64)LAT_TILES * ETILE;
+      if (p.k(r, h) == 0) continue;
+      lat = p.F(r, h) <= (i64)LAT_TILES * NT && p.E(r, h) <= (i64)LAT_TILES * ETILE;
     }
-  const bool p2p = sharded && shard->exchange != nullptr;
-  bool v2 = !lat && !synced && !nodedup && !disjoint && !any_time && L > 0 && (!sharded || p2p) && (!no_v2 || p2p || weighted);
-  std::vector<i64> type_nodes((size_t)T, -1);   // nodes of each type, where a relation with that source type tells us
-  for (int r = 0; r < R; ++r) type_nodes[rels[r].src_type] = std::max(type_nodes[rels[r].src_type], (i64)rels[r].num_src_nodes);
+  const bool p2p = p.p2p = sharded && shard->exchange != nullptr;
+  bool& v2 = p.v2;
+  v2 = !lat && !synced && !nodedup && !disjoint && !any_time && L > 0 && (!sharded || p2p) && (!no_v2 || p2p || p.weighted);
+  p.type_nodes.assign((size_t)T, -1);
+  for (int r = 0; r < R; ++r) p.type_nodes[rels[r].src_type] = std::max(p.type_nodes[rels[r].src_type], (i64)rels[r].num_src_nodes);
   if (v2)   // every node type's id range must be known and fit the packed key (a type that is never a source has no bound)
-    for (int t = 0; t < T && v2; ++t) v2 = idx32 || (type_nodes[t] >= 0 && type_nodes[t] < 0xffffffffll);
+    for (int t = 0; t < T && v2; ++t) v2 = idx32 || (p.type_nodes[t] >= 0 && p.type_nodes[t] < 0xffffffffll);
   if (p2p) PYGB_CHECK(v2 && T == 1 && R == 1 && shard->world <= V2_MAX_W, PYGB200_ERR_UNSUPPORTED,
                       "peer-memory frontier sharding: homogeneous, non-disjoint, bounded fan-outs, node ids < 2^32-1, world <= 16");
-  if (weighted) PYGB_CHECK(!sharded, PYGB200_ERR_UNSUPPORTED, "biased sampling is not frontier-sharded: one GPU per batch");
-  const int XW = p2p ? shard->world : 1, XR = p2p ? shard->rank : 0;
+  if (p.weighted) PYGB_CHECK(!sharded, PYGB200_ERR_UNSUPPORTED, "biased sampling is not frontier-sharded: one GPU per batch");
+  p.XW = p2p ? shard->world : 1;
+  p.XR = p2p ? shard->rank : 0;
 
   // ---- results straight into the caller's arrays?  (bounded int64 non-disjoint runs only; the binding is one-shot)
-  bool direct = bound_armed && !synced && (!sharded || shard->exchange != nullptr) && !nodedup && !idx32 && !disjoint &&
-                (int)s->bound.node.size() == T && (int)s->bound.row.size() == R;
-  for (int t = 0; t < T && direct; ++t) direct = s->bound.node[t] != nullptr && s->bound.ncap[t] >= node_cap[t];
+  bool& direct = p.direct;
+  direct = bound_armed && !synced && (!sharded || shard->exchange != nullptr) && !nodedup && !idx32 && !disjoint &&
+           (int)s->bound.node.size() == T && (int)s->bound.row.size() == R;
+  for (int t = 0; t < T && direct; ++t) direct = s->bound.node[t] != nullptr && s->bound.ncap[t] >= p.node_cap[t];
   for (int r = 0; r < R && direct; ++r)
-    direct = s->bound.row[r] != nullptr && s->bound.col[r] != nullptr && s->bound.ecap[r] >= rel_cap[r];
+    direct = s->bound.row[r] != nullptr && s->bound.col[r] != nullptr && s->bound.ecap[r] >= p.rel_cap[r];
+
+  // the first pass that will run (hop 0) is counted inside the seed launch of its source type (extra blocks)
+  if (lat)
+    for (int r = 0; r < R; ++r)
+      if (p.launches(r, 0)) { p.fuse_r = r; p.fuse_t = rels[r].src_type; break; }
+  return PYGB200_OK;
+}
+
+// ------------------------------------------------------------------------------------- run
+// latency schedule: a counter is the write-once word st[w] (w >= 0), else the constant c
+struct Wd { int w; i64 c; };
+
+// One run: its state, and one member function per phase (sampler_run_impl calls them in order).  idx_t is the index type
+// of the caller's seeds and CSR (PYGB200_S_INDEX32); every kernel that reads them is launched as its idx_t instance.
+template <typename idx_t>
+struct Run {
+  pygb200_sampler* s;
+  cudaStream_t st;
+  const RunPlan& p;
+  Layout lay{};
+  i64* dst = nullptr;         // this run's half of the device state
+  i64* dst_other = nullptr;   // the other half (cleared by whoever publishes the run, for the next one)
+  i64 out0 = 0;               // raw index of this run's first engine output
+  i64 raw_cap = 0;            // raw stream capacity (words) the kernels are given
+  i64 run_outputs = 0, run_outputs_max = 0;   // see mt_stream
+  i64 wwords = 0;             // engine outputs consumed by biased passes so far
+  i64 eng_blocks_max = 1;     // mixed: upper bound of the RandintEngine blocks fetched so far
+  // lookup of the last pass, deferred into the next k_count / the final kernel
+  i64* lk_colv = nullptr; const u64* lk_vals = nullptr; i64 lk_E = 0;
+  // latency schedule: the static pass schedule decides which write-once word holds what
+  std::vector<Wd> cur_list, sl_begin, sl_end, relcum, list_end;
+  std::vector<int> eph_w;
+  Wd cursor{-1, 0};
+  int lk_w_E = -1, lk_w_pbase = -1;
+  bool published = false;   // the last pass publishes the run (else k_final does)
+  int pub_w_list = -1;      // the counter that arrives as the flag word's payload
 
   // ---- workspace
-  if (s->cleanup_pending && !s->types.empty() && s->types[0].tcap) {   // nobody exported the previous run: reset its table now
-    auto& tb = s->types[0];
-    launch_pdl(k_cleanup, grid_for((i64)(tb.slot.cap / 4), NT, s->sm_count), NT, 0, st, tb.keys.as<u64>(), tb.vals.as<u64>(),
-               (const u32*)tb.slot.as<u32>(), (const i64*)(s->st_last + s->st_o_list));
-    PYGB_LAUNCH_CHECK();
-    s->cleanup_pending = false;
-  }
-  if ((int)s->types.size() < T) s->types.resize(T);
-  if ((int)s->rels.size() < R) s->rels.resize(R);
-  s->T = T; s->R = R; s->L = L; s->disjoint = disjoint;
-  const Layout lay = make_layout(T, R, L);
-  if (lay.words > s->st_words) {
-    if (s->st_host) cudaFreeHost(s->st_host);
-    s->st_host = nullptr; s->st_words = 0;
-    PYGB_CUDA(cudaHostAlloc((void**)&s->st_host, (lay.words + 8) * 8, cudaHostAllocMapped));
-    PYGB_CUDA(cudaHostGetDevicePointer((void**)&s->st_host_dev, s->st_host, 0));
-    memset(s->st_host, 0, (lay.words + 8) * 8);
-    s->st_words = lay.words;
-  }
-  if (int e = s->st.ensure(2 * lay.words * 8, 0, st)) return e;
-  if (int e = s->gen.ensure(64, 0, st)) return e;
-  if (!s->mt_stream) {
-    PYGB_CUDA(cudaStreamCreateWithFlags(&s->mt_stream, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; ++i) PYGB_CUDA(cudaEventCreateWithFlags(&s->mt_ev[i], cudaEventDisableTiming));
-    PYGB_CUDA(cudaEventCreateWithFlags(&s->mt_order_ev, cudaEventDisableTiming));
-  }
-  if (s->dirty) {  // previous run aborted: wipe tables, forget the stream
-    for (auto& tb : s->types) if (tb.tcap) {
-      PYGB_CUDA(cudaMemsetAsync(tb.keys.p, 0xff, tb.tcap * 8, st));
-      PYGB_CUDA(cudaMemsetAsync(tb.vals.p, 0xff, tb.tcap * 8, st));
+  int workspace() {
+    const int T = p.T, R = p.R, L = p.L;
+    if (s->cleanup_pending && !s->types.empty() && s->types[0].tcap) {   // nobody exported the previous run: reset its table now
+      if (int e = cleanup_table(0, (i64)(s->types[0].slot.cap / 4), s->st_last + s->st_o_list)) return e;
+      s->cleanup_pending = false;
     }
-    for (int i = 0; i < 2; ++i) if (s->clean_pending[i]) { PYGB_CUDA(cudaStreamWaitEvent(st, s->clean_done[i], 0)); s->clean_pending[i] = false; }
-    for (auto& tb : s->types)
-      for (int i = 0; i < 2; ++i) if (tb.pk_bits[i]) PYGB_CUDA(cudaMemsetAsync(tb.pk[i].p, 0xff, (size_t)8 << tb.pk_bits[i], st));
-    for (int i = 0; i < 2; ++i) if (s->seedpk_bits[i]) PYGB_CUDA(cudaMemsetAsync(s->seedpk[i].p, 0xff, (size_t)8 << s->seedpk_bits[i], st));
-    s->mt_valid = false;
-    s->st_dev_words = 0;
-  }
-  s->dirty = true;
-  if (v2) {
-    if (!s->clean_stream) {
-      PYGB_CUDA(cudaStreamCreateWithFlags(&s->clean_stream, cudaStreamNonBlocking));
-      for (int i = 0; i < 2; ++i) PYGB_CUDA(cudaEventCreateWithFlags(&s->clean_done[i], cudaEventDisableTiming));
-      PYGB_CUDA(cudaEventCreateWithFlags(&s->final_ev, cudaEventDisableTiming));
+    if ((int)s->types.size() < T) s->types.resize(T);
+    if ((int)s->rels.size() < R) s->rels.resize(R);
+    s->T = T; s->R = R; s->L = L; s->disjoint = p.disjoint;
+    lay = make_layout(T, R, L);
+    if (lay.words > s->st_words) {
+      if (s->st_host) cudaFreeHost(s->st_host);
+      s->st_host = nullptr; s->st_words = 0;
+      PYGB_CUDA(cudaHostAlloc((void**)&s->st_host, (lay.words + 8) * 8, cudaHostAllocMapped));
+      PYGB_CUDA(cudaHostGetDevicePointer((void**)&s->st_host_dev, s->st_host, 0));
+      memset(s->st_host, 0, (lay.words + 8) * 8);
+      s->st_words = lay.words;
     }
-    s->v2_side ^= 1;   // the other table: the previous v2 run's one may still be resetting on the side stream
-    if (s->clean_pending[s->v2_side]) { PYGB_CUDA(cudaStreamWaitEvent(st, s->clean_done[s->v2_side], 0)); s->clean_pending[s->v2_side] = false; }
-    for (int t = 0; t < T; ++t) {
-      if (int e = ensure_type(s, t, node_cap[t], 0, false, st)) return e;
-      // distinct keys <= min(static bound, nodes of the type): a products-sized graph (2.4 M nodes) keeps its table
-      // L2-resident (64 MB) whatever the batch; a rank's table holds the keys it owns: 1/W of them (+25 % for imbalance)
-      const i64 keys = type_nodes[t] >= 0 ? std::min(node_cap[t], type_nodes[t]) : node_cap[t];
-      if (int e = ensure_table_v2(s, t, s->v2_side, XW == 1 ? keys : keys / XW + keys / (4 * XW) + 1024, node_cap[t], st)) return e;
+    if (int e = s->st.ensure(2 * lay.words * 8, 0, st)) return e;
+    if (int e = s->gen.ensure(64, 0, st)) return e;
+    if (!s->mt_stream) {
+      PYGB_CUDA(cudaStreamCreateWithFlags(&s->mt_stream, cudaStreamNonBlocking));
+      for (int i = 0; i < 2; ++i) PYGB_CUDA(cudaEventCreateWithFlags(&s->mt_ev[i], cudaEventDisableTiming));
+      PYGB_CUDA(cudaEventCreateWithFlags(&s->mt_order_ev, cudaEventDisableTiming));
     }
-    for (int r = 0; r < R; ++r) if (int e = ensure_rel(s, r, rel_cap[r], 0, st)) return e;
-    if (int e = ensure_frontier_scratch(s, max_F, st)) return e;
-    if (int e = ensure_edge_scratch(s, max_E, st)) return e;
-    if (p2p) {
-      if (int e = ensure_xregion(s, max_E, shard, st)) return e;
-      int bits = 10;
-      while ((1ull << bits) < 2 * (u64)std::max<i64>(total_seeds, 1)) ++bits;
-      if (bits > s->seedpk_bits[s->v2_side]) {
-        if (int e = s->seedpk[s->v2_side].ensure((size_t)8 << bits, 0, st)) return e;
-        PYGB_CUDA(cudaMemsetAsync(s->seedpk[s->v2_side].p, 0xff, (size_t)8 << bits, st));
-        s->seedpk_bits[s->v2_side] = bits;
+    if (s->dirty) {  // previous run aborted: wipe tables, forget the stream
+      for (auto& tb : s->types) if (tb.tcap) {
+        PYGB_CUDA(cudaMemsetAsync(tb.keys.p, 0xff, tb.tcap * 8, st));
+        PYGB_CUDA(cudaMemsetAsync(tb.vals.p, 0xff, tb.tcap * 8, st));
       }
-    } else if (int e = s->fref.ensure((size_t)max_E * 4, 0, st)) return e;
-  } else if (!synced) {
-    for (int t = 0; t < T; ++t) {
-      if (int e = ensure_type(s, t, node_cap[t], 0, disjoint, st)) return e;
-      if (int e = ensure_table(s, t, node_cap[t], 0, st)) return e;
+      for (int i = 0; i < 2; ++i) if (s->clean_pending[i]) { PYGB_CUDA(cudaStreamWaitEvent(st, s->clean_done[i], 0)); s->clean_pending[i] = false; }
+      for (auto& tb : s->types)
+        for (int i = 0; i < 2; ++i) if (tb.pk_bits[i]) PYGB_CUDA(cudaMemsetAsync(tb.pk[i].p, 0xff, (size_t)8 << tb.pk_bits[i], st));
+      for (int i = 0; i < 2; ++i) if (s->seedpk_bits[i]) PYGB_CUDA(cudaMemsetAsync(s->seedpk[i].p, 0xff, (size_t)8 << s->seedpk_bits[i], st));
+      s->mt_valid = false;
+      s->st_dev_words = 0;
     }
-    for (int r = 0; r < R; ++r) if (int e = ensure_rel(s, r, rel_cap[r], 0, st)) return e;
-    if (int e = ensure_frontier_scratch(s, max_F, st)) return e;
-    if (int e = ensure_edge_scratch(s, max_E, st)) return e;
-  } else {
-    for (int t = 0; t < T; ++t) {
-      if (int e = ensure_type(s, t, std::max<i64>(n_seeds[t], 1), 0, disjoint, st)) return e;
-      if (int e = ensure_table(s, t, std::max<i64>(n_seeds[t], 1), 0, st)) return e;
+    s->dirty = true;
+    if (p.v2) {
+      if (!s->clean_stream) {
+        PYGB_CUDA(cudaStreamCreateWithFlags(&s->clean_stream, cudaStreamNonBlocking));
+        for (int i = 0; i < 2; ++i) PYGB_CUDA(cudaEventCreateWithFlags(&s->clean_done[i], cudaEventDisableTiming));
+        PYGB_CUDA(cudaEventCreateWithFlags(&s->final_ev, cudaEventDisableTiming));
+      }
+      s->v2_side ^= 1;   // the other table: the previous v2 run's one may still be resetting on the side stream
+      if (s->clean_pending[s->v2_side]) { PYGB_CUDA(cudaStreamWaitEvent(st, s->clean_done[s->v2_side], 0)); s->clean_pending[s->v2_side] = false; }
+      for (int t = 0; t < T; ++t) {
+        if (int e = ensure_type(s, t, p.node_cap[t], 0, false, st)) return e;
+        // distinct keys <= min(static bound, nodes of the type): a products-sized graph (2.4 M nodes) keeps its table
+        // L2-resident (64 MB) whatever the batch; a rank's table holds the keys it owns: 1/W of them (+25 % for imbalance)
+        const i64 keys = p.type_nodes[t] >= 0 ? std::min(p.node_cap[t], p.type_nodes[t]) : p.node_cap[t];
+        const i64 own = p.XW == 1 ? keys : keys / p.XW + keys / (4 * p.XW) + 1024;
+        if (int e = ensure_table_v2(s, t, s->v2_side, own, p.node_cap[t], st)) return e;
+      }
+      for (int r = 0; r < R; ++r) if (int e = ensure_rel(s, r, p.rel_cap[r], 0, st)) return e;
+      if (int e = ensure_frontier_scratch(s, p.max_F, st)) return e;
+      if (int e = ensure_edge_scratch(s, p.max_E, st)) return e;
+      if (p.p2p) {
+        if (int e = ensure_xregion(s, p.max_E, p.shard, st)) return e;
+        int bits = 10;
+        while ((1ull << bits) < 2 * (u64)std::max<i64>(p.total_seeds, 1)) ++bits;
+        if (bits > s->seedpk_bits[s->v2_side]) {
+          if (int e = s->seedpk[s->v2_side].ensure((size_t)8 << bits, 0, st)) return e;
+          PYGB_CUDA(cudaMemsetAsync(s->seedpk[s->v2_side].p, 0xff, (size_t)8 << bits, st));
+          s->seedpk_bits[s->v2_side] = bits;
+        }
+      } else if (int e = s->fref.ensure((size_t)p.max_E * 4, 0, st)) return e;
+    } else if (!p.synced) {
+      for (int t = 0; t < T; ++t) {
+        if (int e = ensure_type(s, t, p.node_cap[t], 0, p.disjoint, st)) return e;
+        if (int e = ensure_table(s, t, p.node_cap[t], 0, st)) return e;
+      }
+      for (int r = 0; r < R; ++r) if (int e = ensure_rel(s, r, p.rel_cap[r], 0, st)) return e;
+      if (int e = ensure_frontier_scratch(s, p.max_F, st)) return e;
+      if (int e = ensure_edge_scratch(s, p.max_E, st)) return e;
+    } else {
+      for (int t = 0; t < T; ++t) {
+        if (int e = ensure_type(s, t, std::max<i64>(p.n_seeds[t], 1), 0, p.disjoint, st)) return e;
+        if (int e = ensure_table(s, t, std::max<i64>(p.n_seeds[t], 1), 0, st)) return e;
+      }
+      for (int r = 0; r < R; ++r) if (int e = ensure_rel(s, r, 1, 0, st)) return e;
+      if (int e = ensure_edge_scratch(s, p.total_seeds, st)) return e;
     }
-    for (int r = 0; r < R; ++r) if (int e = ensure_rel(s, r, 1, 0, st)) return e;
-    if (int e = ensure_edge_scratch(s, total_seeds, st)) return e;
+    return PYGB200_OK;
   }
 
   // ---- mt19937 raw stream: continue the persistent one or (re)start from the caller's engine state.
@@ -1932,86 +2000,112 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
   //                   frontier node has >= 2^16 neighbours); pre-generation targets use it, a shortfall is
   //                   extended by the last block of k_count;
   // run_outputs_max : the worst case (32/64-bit draws incl. skipped units), used only for capacity.
-  const i64 run_outputs = synced ? 256 * 2 : 256 * (rng_blocks_for_units(draw_count) + 1);
-  const i64 run_outputs_max = synced ? 256 * 2 : 256 * (rng_blocks_for_units(draw_units) + 1);
-  auto wait_all_pregen = [&]() -> int {
+  int wait_all_pregen() {
     for (int i = 0; i < 2; ++i) if (s->mt_ev_pending[i]) { PYGB_CUDA(cudaStreamWaitEvent(st, s->mt_ev[i], 0)); s->mt_ev_pending[i] = false; }
     return PYGB200_OK;
-  };
-  i64 out0;
-  bool cont = s->mt_valid && memcmp(&s->mt_expected, mt, sizeof(*mt)) == 0 &&
-              s->mt_q + run_outputs_max + run_outputs + 6 * MT_N <= s->raw_cap_words;
-  if (synced || weighted) {  // these runs extend the stream themselves (k_count / between passes): nothing may run beside them
-    if (int e = wait_all_pregen()) return e;
-    s->mt_gen_known = 0;
   }
-  if (!cont || synced || weighted) s->mt_defer_target = 0;
-  if (cont) {
-    out0 = s->mt_q;
-    const i64 need = out0 + run_outputs + MT_N;
-    // oldest pending launch that covers this run (mt_ev_next is the older slot)
-    const int older = s->mt_ev_next, newer = s->mt_ev_next ^ 1;
-    if (s->mt_gen_known >= need) {
-      // covered by a launch this stream has already waited for; newer launches keep running beside us
-    } else if (s->mt_ev_pending[older] && s->mt_ev_target[older] >= need) {
-      PYGB_CUDA(cudaStreamWaitEvent(st, s->mt_ev[older], 0));
-      s->mt_ev_pending[older] = false;
-      s->mt_gen_known = std::max(s->mt_gen_known, s->mt_ev_target[older]);
-    } else if (s->mt_ev_pending[newer] && s->mt_ev_target[newer] >= need) {
-      // same side stream: once the newer launch is complete so is the older one
-      PYGB_CUDA(cudaStreamWaitEvent(st, s->mt_ev[newer], 0));
-      s->mt_ev_pending[older] = s->mt_ev_pending[newer] = false;
-      s->mt_gen_known = std::max(s->mt_gen_known, s->mt_ev_target[newer]);
-    } else {
-      // not covered ahead of time (first continued run, or a run larger than the previous one): extend here
+  int mt_stream(const pygb200_mt19937* mt) {
+    const bool synced = p.synced, weighted = p.weighted;
+    run_outputs = synced ? 256 * 2 : 256 * (rng_blocks_for_units(p.draw_count) + 1);
+    run_outputs_max = synced ? 256 * 2 : 256 * (rng_blocks_for_units(p.draw_units) + 1);
+    bool cont = s->mt_valid && memcmp(&s->mt_expected, mt, sizeof(*mt)) == 0 &&
+                s->mt_q + run_outputs_max + run_outputs + 6 * MT_N <= s->raw_cap_words;
+    if (synced || weighted) {  // these runs extend the stream themselves (k_count / between passes): nothing may run beside them
       if (int e = wait_all_pregen()) return e;
-      if (int e = mt_request(s, st, need)) return e;
-      s->mt_gen_known = need;
-      // the side stream continues from here: order its next launch behind this one
-      PYGB_CUDA(cudaEventRecord(s->mt_order_ev, st));
-      PYGB_CUDA(cudaStreamWaitEvent(s->mt_stream, s->mt_order_ev, 0));
+      s->mt_gen_known = 0;
     }
-  } else {
-    if (int e = wait_all_pregen()) return e;
-    static const i64 pref_cap = [] { const char* e = getenv("PYGB200_MT_CAP_WORDS"); return e ? (i64)atoll(e) : (i64)1 << 23; }();
-    load_jump_table(s, st);
-    const i64 want = std::max<i64>((i64)MT_N + 4 * (run_outputs_max + run_outputs) + 8 * MT_N + 2 * (i64)s->jump_S, pref_cap);  // default 32 MB of raw words
-    if (want > s->raw_cap_words) {
-      if (int e = s->raw.ensure((size_t)want * 4, 0, st)) return e;
-      s->raw_cap_words = want;
+    if (!cont || synced || weighted) s->mt_defer_target = 0;
+    if (cont) {
+      out0 = s->mt_q;
+      const i64 need = out0 + run_outputs + MT_N;
+      // oldest pending launch that covers this run (mt_ev_next is the older slot)
+      const int older = s->mt_ev_next, newer = s->mt_ev_next ^ 1;
+      if (s->mt_gen_known >= need) {
+        // covered by a launch this stream has already waited for; newer launches keep running beside us
+      } else if (s->mt_ev_pending[older] && s->mt_ev_target[older] >= need) {
+        PYGB_CUDA(cudaStreamWaitEvent(st, s->mt_ev[older], 0));
+        s->mt_ev_pending[older] = false;
+        s->mt_gen_known = std::max(s->mt_gen_known, s->mt_ev_target[older]);
+      } else if (s->mt_ev_pending[newer] && s->mt_ev_target[newer] >= need) {
+        // same side stream: once the newer launch is complete so is the older one
+        PYGB_CUDA(cudaStreamWaitEvent(st, s->mt_ev[newer], 0));
+        s->mt_ev_pending[older] = s->mt_ev_pending[newer] = false;
+        s->mt_gen_known = std::max(s->mt_gen_known, s->mt_ev_target[newer]);
+      } else {
+        // not covered ahead of time (first continued run, or a run larger than the previous one): extend here
+        if (int e = wait_all_pregen()) return e;
+        if (int e = mt_request(s, st, need)) return e;
+        s->mt_gen_known = need;
+        // the side stream continues from here: order its next launch behind this one
+        PYGB_CUDA(cudaEventRecord(s->mt_order_ev, st));
+        PYGB_CUDA(cudaStreamWaitEvent(s->mt_stream, s->mt_order_ev, 0));
+      }
+    } else {
+      if (int e = wait_all_pregen()) return e;
+      static const i64 pref_cap = [] { const char* e = getenv("PYGB200_MT_CAP_WORDS"); return e ? (i64)atoll(e) : (i64)1 << 23; }();
+      load_jump_table(s, st);
+      const i64 want = std::max<i64>((i64)MT_N + 4 * (run_outputs_max + run_outputs) + 8 * MT_N + 2 * (i64)s->jump_S, pref_cap);  // default 32 MB of raw words
+      if (want > s->raw_cap_words) {
+        if (int e = s->raw.ensure((size_t)want * 4, 0, st)) return e;
+        s->raw_cap_words = want;
+      }
+      MTPodParam pod;
+      memcpy(pod.state, mt->state, sizeof(pod.state));
+      if (int e = launch<PLAIN>(nullptr, 0, k_mt_init, 1, NT, 0, st, s->raw.as<u32>(), s->gen.as<i64>(), pod)) return e;
+      out0 = mt_next0(mt->left);
+      s->mt_gen_known = MT_N;
+      s->mt_requested = MT_N;
+      if (!synced) {  // cover this run's expected need up front so that no pass has to extend the stream itself
+        if (int e = mt_request(s, st, out0 + run_outputs + MT_N)) return e;
+        s->mt_gen_known = out0 + run_outputs + MT_N;
+      }
     }
-    MTPodParam pod;
-    memcpy(pod.state, mt->state, sizeof(pod.state));
-    k_mt_init<<<1, NT, 0, st>>>(s->raw.as<u32>(), s->gen.as<i64>(), pod);
-    PYGB_LAUNCH_CHECK();
-    out0 = mt_next0(mt->left);
-    s->mt_gen_known = MT_N;
-    s->mt_requested = MT_N;
-    if (!synced) {  // cover this run's expected need up front so that no pass has to extend the stream itself
-      if (int e = mt_request(s, st, out0 + run_outputs + MT_N)) return e;
-      s->mt_gen_known = out0 + run_outputs + MT_N;
+    s->mt_valid = false;  // until this run completes
+    raw_cap = s->raw_cap_words;
+    if (p.mixed) {   // the engine's first block (fetched by its constructor, before anything else draws) opens the compacted copy
+      if (int e = mt_request(s, st, out0 + 512 + MT_N)) return e;
+      if (int e = s->eraw.ensure(512 * 4, 0, st)) return e;
+      PYGB_CUDA(cudaMemcpyAsync(s->eraw.p, s->raw.as<u32>() + out0, 256 * 4, cudaMemcpyDeviceToDevice, st));
     }
+    return PYGB200_OK;
   }
-  s->mt_valid = false;  // until this run completes
-  i64 raw_cap = s->raw_cap_words;
-  if (mixed) {   // the engine's first block (fetched by its constructor, before anything else draws) opens the compacted copy
-    if (int e = mt_request(s, st, out0 + 512 + MT_N)) return e;
-    if (int e = s->eraw.ensure(512 * 4, 0, st)) return e;
-    PYGB_CUDA(cudaMemcpyAsync(s->eraw.p, s->raw.as<u32>() + out0, 256 * 4, cudaMemcpyDeviceToDevice, st));
+
+  // The raw stream buffer grows to `need` words, keeping what has been generated.
+  int grow_raw(i64 need) {
+    i64 gen_now = 0;
+    PYGB_CUDA(cudaMemcpyAsync(&gen_now, s->gen.p, 8, cudaMemcpyDeviceToHost, st));
+    PYGB_CUDA(cudaStreamSynchronize(st));
+    if (int e = s->raw.ensure((size_t)need * 4, (size_t)gen_now * 4, st)) return e;
+    raw_cap = s->raw_cap_words = (i64)(s->raw.cap / 4);
+    return PYGB200_OK;
   }
 
   // ---- init: zero state.  Two halves: the previous run's k_final already cleared the one this run uses.
-  if (s->st_dev_words != lay.words) {
-    PYGB_CUDA(cudaMemsetAsync(s->st.p, 0, 2 * lay.words * 8, st));
-    s->st_dev_words = lay.words;
-    s->st_cur = 0;
-  } else {
-    s->st_cur ^= 1;
+  int init_state() {
+    if (s->st_dev_words != lay.words) {
+      PYGB_CUDA(cudaMemsetAsync(s->st.p, 0, 2 * lay.words * 8, st));
+      s->st_dev_words = lay.words;
+      s->st_cur = 0;
+    } else {
+      s->st_cur ^= 1;
+    }
+    dst = s->st.as<i64>() + (size_t)s->st_cur * lay.words;
+    dst_other = s->st.as<i64>() + (size_t)(s->st_cur ^ 1) * lay.words;
+    s->st_last = dst;
+    if (p.weighted && !s->wl_ready) {   // biased sampling: MKL logf deviations, once per sampler
+      if (int e = s->wl_tab.ensure(sizeof(kMklLogfTable), 0, st)) return e;
+      if (int e = s->wl_bits.ensure((size_t)1 << 21, 0, st)) return e;
+      PYGB_CUDA(cudaMemcpyAsync(s->wl_tab.p, kMklLogfTable, sizeof(kMklLogfTable), cudaMemcpyHostToDevice, st));
+      PYGB_CUDA(cudaMemsetAsync(s->wl_bits.p, 0, (size_t)1 << 21, st));
+      if (int e = launch<PLAIN>(nullptr, 0, k_w_log_bitmap, ceil_div(kMklLogfTableN, NT), NT, 0, st, s->wl_tab.as<u32>(), kMklLogfTableN,
+                                s->wl_bits.as<u32>()))
+        return e;
+      s->wl_ready = true;
+    }
+    return PYGB200_OK;
   }
-  i64* dst = s->st.as<i64>() + (size_t)s->st_cur * lay.words;
-  i64* dst_other = s->st.as<i64>() + (size_t)(s->st_cur ^ 1) * lay.words;
-  s->st_last = dst;
-  auto make_args = [&](int src_t, int dst_t, int rel) {
+
+  PassArgs make_args(int src_t, int dst_t, int rel) const {
     PassArgs a;
     memset(&a, 0, sizeof(a));
     auto& td = s->types[dst_t];
@@ -2019,11 +2113,11 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
     a.keys = td.keys.as<u64>(); a.vals = td.vals.as<u64>(); a.mask = td.tcap - 1;
     if (src_t >= 0) { a.src_nodes = s->types[src_t].nodes.as<i64>(); a.src_batch = s->types[src_t].batch.as<i64>(); }
     if (rel >= 0) {
-      a.rowptr = rels[rel].rowptr; a.col = rels[rel].col;
+      a.rowptr = p.rels[rel].rowptr; a.col = p.rels[rel].col;
       a.row = s->rels[rel].row.as<i64>(); a.colv = s->rels[rel].colv.as<i64>(); a.eid = s->rels[rel].eid.as<i64>();
       a.o_rel_edges = lay.o_rel + rel;
     }
-    if (direct) {
+    if (p.direct) {
       a.dst_nodes = s->bound.node[dst_t];
       if (src_t >= 0) a.src_nodes = s->bound.node[src_t];
       if (rel >= 0) {
@@ -2038,113 +2132,121 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
     a.o_src_begin = lay.o_begin + (src_t >= 0 ? src_t : 0); a.o_src_end = lay.o_end + (src_t >= 0 ? src_t : 0);
     a.o_dst_list = lay.o_list + dst_t; a.o_dst_ids = lay.o_ids + dst_t;
     a.raw = s->raw.as<u32>(); a.gen = s->gen.as<i64>(); a.out0 = out0; a.raw_cap = raw_cap;
-    a.replace = replace; a.disjoint = disjoint;
-    if (v2) {
+    a.replace = p.replace; a.disjoint = p.disjoint;
+    if (p.v2) {
       a.pk = td.pk[s->v2_side].as<u64>(); a.pk_bits = td.pk_bits[s->v2_side];
       a.dst_slot = td.vslot[s->v2_side].as<u32>();
-      a.xw = XW; a.xr = XR; a.o_shard = lay.o_shard;
+      a.xw = p.XW; a.xr = p.XR; a.o_shard = lay.o_shard;
       a.fref = s->fref.as<u32>();
-      if (p2p) {
+      if (p.p2p) {
         const auto& x = s->x;
-        for (int q = 0; q < XW; ++q) a.xpeer[q] = x.peer[q];
+        for (int q = 0; q < p.XW; ++q) a.xpeer[q] = x.peer[q];
         a.x_off_bar = x.off_bar; a.x_off_fref = x.off_fref;
         a.x_off_exc = x.off_exc; a.x_off_exc_n = x.off_exc_n; a.x_off_xcnt = x.off_xcnt; a.x_exc_cap = x.cap;
         a.x_off_dst = x.off_dst[x.passes & 1]; a.x_off_eid = x.off_eid[x.passes & 1];
         a.fref = reinterpret_cast<u32*>(x.base + x.off_fref);
-        a.x_eid64 = (rel >= 0 && rels[rel].num_edges > 0xffffffffll) ? 1 : 0;
+        a.x_eid64 = (rel >= 0 && p.rels[rel].num_edges > 0xffffffffll) ? 1 : 0;
       }
     }
-    if (any_time && rel >= 0) {  // edge time of the relation wins over node time of its dst type (:742-787)
+    if (p.any_time && rel >= 0) {  // edge time of the relation wins over node time of its dst type (:742-787)
+      const pygb200_temporal* temporal = p.temporal;
       if (temporal->edge_time && temporal->edge_time[rel]) { a.time_mode = 2; a.time = reinterpret_cast<const i64*>(temporal->edge_time[rel]); }
       else if (temporal->node_time && temporal->node_time[dst_t]) { a.time_mode = 1; a.time = reinterpret_cast<const i64*>(temporal->node_time[dst_t]); }
       a.seed_times = s->seed_times.as<i64>();
       a.time_last = temporal->strategy_last;
     }
     return a;
-  };
-  auto read_state = [&]() -> int {
+  }
+  // the arguments of pass (hop h, relation r); mixed runs point the uniform relations at the compacted engine blocks
+  PassArgs pass_args(int r, int h) const {
+    PassArgs a = make_args(p.rels[r].src_type, p.rels[r].dst_type, r);
+    a.fanout = p.k(r, h);
+    a.o_eph = lay.o_eph + r * p.L + h;
+    if (p.mixed && !p.wrel[r]) { a.raw = s->eraw.as<u32>(); a.out0 = 0; a.raw_cap = (i64)(s->eraw.cap / 4); }
+    return a;
+  }
+  // the last pass of hop h folds the end-of-hop bookkeeping into its k_mark
+  void with_hop_end(PassArgs& a, int h) const {
+    a.he_T = p.T; a.he_L = p.L; a.he_hop = h; a.he_list = lay.o_list; a.he_begin = lay.o_begin; a.he_end = lay.o_end;
+    a.he_nph = lay.o_nph;
+  }
+  // the same, standalone, for a hop whose last pass did not run it
+  int hop_end(int h) { return launch<PLAIN>(nullptr, 0, k_hop_end, 1, 1024, 0, st, dst, p.T, p.L, h, lay.o_list, lay.o_begin, lay.o_end, lay.o_nph); }
+  int read_state() {
     PYGB_CUDA(cudaMemcpyAsync(s->st_host, dst, lay.words * 8, cudaMemcpyDeviceToHost, st));
     PYGB_CUDA(cudaStreamSynchronize(st));
     return PYGB200_OK;
-  };
+  }
 
-  // v2: from the inserts of a pass (or of the seeds) to ids.  Single GPU: mark reads the refs from the table.
+  // a count kernel's grid: F frontier nodes, and the deferred lookup of the previous pass (E_prev edges)
+  int count_grid(const PassArgs& a, i64 F, i64 E_prev) const {
+    return std::max(grid_for(F, NT, s->sm_count), a.lk_colv ? grid_for(E_prev, NT, s->sm_count) : 1);
+  }
+  // the publication of the run's counters and engine state to the host (by k_final, or the latency schedule's last pass)
+  void publish(PassArgs& a) const {
+    a.pub_host = s->st_host_dev; a.pub_zero = dst_other; a.pub_serial = s->run_serial; a.pub_words = (int)lay.words;
+    a.pub_o_mt = lay.o_mt;
+  }
+
+  // ---- the wide-table pass kernels
+  int count(const PassArgs& a, i64 F, i64 E_prev) { return launch<PDL>("count", F, k_count<idx_t>, count_grid(a, F, E_prev), NT, 0, st, a); }
+  int sample(const PassArgs& a_in, i64 F, i64 E) {
+    PassArgs a = a_in;
+    a.group = sample_group_lanes(a.fanout);
+    return launch<PDL>("sample", E, k_sample<idx_t>, grid_for(F, sample_nodes_per_block(a.group), s->sm_count), NT, 0, st, a);
+  }
+  int rest(const PassArgs& a, i64 F, i64 E, bool lookup_now, bool with_sample = true) {
+    if (with_sample) if (int e = sample(a, F, E)) return e;
+    if (int e = launch<PDL>("mark", E, k_mark, grid_for(E, ETILE, s->sm_count), NT, 0, st, a)) return e;
+    if (int e = launch<PDL>("assign", E, k_assign, grid_for(E, NT, s->sm_count), NT, 0, st, a)) return e;
+    if (lookup_now) return launch<PLAIN>("lookup", E, k_lookup, grid_for(E, NT, s->sm_count), NT, 0, st, a);
+    return PYGB200_OK;
+  }
+  // a pass whose edge ids are already drawn (biased draws, all-gathered shards): expand from them (gather col, rows, hash
+  // insert), then mark / assign
+  int expand(const PassArgs& a, i64 F, i64 E, bool lookup_now) {
+    PassArgs d = a;
+    d.phase = 2;
+    if (int e = sample(d, F, E)) return e;
+    return rest(a, F, E, lookup_now, false);
+  }
+
+  // ---- v2: from the inserts of a pass (or of the seeds) to ids.  Single GPU: mark reads the refs from the table.
   // Sharded: refs of owned positions -> barrier -> slice-wise reduction over the peers, result stored to all ->
   // barrier -> the same mark on the full ref array.  Then ids (replicated, streaming).
-  static const u64 xbar_timeout_ns = [] { const char* e = getenv("PYGB200_XBARRIER_TIMEOUT_MS"); return (u64)(e ? atoll(e) : 20000) * 1000000ull; }();
-  auto xbarrier = [&](const PassArgs& a) -> int {   // wait until every rank has raised the flags of the current epoch
-    void* tkb = prof_begin(st);
-    launch_pdl(k_xbarrier, 1, 32, 0, st, a, (u64)s->x.epoch, xbar_timeout_ns);
-    prof_end(tkb, "xbarrier", st, 1);
-    PYGB_LAUNCH_CHECK();
-    return PYGB200_OK;
-  };
-  auto v2_ids = [&](const PassArgs& a, i64 Eb) -> int {
-    void* tk;
-    if (p2p) {
+  int xbarrier(const PassArgs& a) {   // wait until every rank has raised the flags of the current epoch
+    return launch<PDL>("xbarrier", 1, k_xbarrier, 1, 32, 0, st, a, (u64)s->x.epoch, xbar_timeout_ns());
+  }
+  int v2_ids(const PassArgs& a, i64 Eb) {
+    if (p.p2p) {
       PassArgs b = a;
-      b.x_timeout_ns = xbar_timeout_ns;
+      b.x_timeout_ns = xbar_timeout_ns();
       b.x_sig_epoch = ++s->x.epoch;   // the last block of k_v2_exc raises the flags ...
-      tk = prof_begin(st);
-      launch_pdl(k_v2_exc, grid_for(Eb, 4 * NT, s->sm_count), NT, 0, st, b);
-      prof_end(tk, "pref", st, Eb);
-      PYGB_LAUNCH_CHECK();
+      if (int e = launch<PDL>("pref", Eb, k_v2_exc, grid_for(Eb, 4 * NT, s->sm_count), NT, 0, st, b)) return e;
       b.x_sig_epoch = 0;
       if (int e = xbarrier(a)) return e;   // ... and k_v2_scatter starts behind everybody's
-      tk = prof_begin(st);
-      PYGB_CUDA(launch_pdl(k_v2_scatter, dim3((unsigned)grid_for(ceil_div(Eb, XW), NT, s->sm_count), (unsigned)XW), NT, 0, st, b));
-      prof_end(tk, "reduce", st, Eb);
-      PYGB_LAUNCH_CHECK();
-      tk = prof_begin(st);
-      launch_pdl(k_v2_mark<false>, grid_for(Eb, ETILE, s->sm_count), NT, 0, st, a);
-    } else {
-      tk = prof_begin(st);
-      launch_pdl(k_v2_mark<true>, grid_for(Eb, ETILE, s->sm_count), NT, 0, st, a);
+      if (int e = launch<PDL>("reduce", Eb, k_v2_scatter, dim3((unsigned)grid_for(ceil_div(Eb, p.XW), NT, s->sm_count), (unsigned)p.XW), NT, 0,
+                              st, b))
+        return e;
+      if (int e = launch<PDL>("mark", Eb, k_v2_mark<false>, grid_for(Eb, ETILE, s->sm_count), NT, 0, st, a)) return e;
+      return launch<PDL>("assign", Eb, k_v2_assign<true>, grid_for(Eb, 4 * NT, s->sm_count), NT, 0, st, a);
     }
-    prof_end(tk, "mark", st, Eb);
-    PYGB_LAUNCH_CHECK();
-    tk = prof_begin(st);
-    if (p2p) launch_pdl(k_v2_assign<true>, grid_for(Eb, 4 * NT, s->sm_count), NT, 0, st, a);
-    else launch_pdl(k_v2_assign<false>, grid_for(Eb, 4 * NT, s->sm_count), NT, 0, st, a);
-    prof_end(tk, "assign", st, Eb);
-    PYGB_LAUNCH_CHECK();
-    return PYGB200_OK;
-  };
+    if (int e = launch<PDL>("mark", Eb, k_v2_mark<true>, grid_for(Eb, ETILE, s->sm_count), NT, 0, st, a)) return e;
+    return launch<PDL>("assign", Eb, k_v2_assign<false>, grid_for(Eb, 4 * NT, s->sm_count), NT, 0, st, a);
+  }
 
   // ---- biased (edge_weight) pass: count -> the host reads the totals (one synchronisation) -> the raw stream and the key
   // scratch are sized -> draws -> inserts -> ids.  The engine outputs of biased passes follow the RandintEngine's first
   // (and, on this path, only) block of 256.
-  i64 wwords = 0;
-  i64 eng_blocks_max = 1;   // mixed: upper bound of the RandintEngine blocks fetched so far
-  auto biased_error = [&](i64 code) -> int {
-    PYGB_CHECK(code != W_ERR_NEG, PYGB200_ERR_ARG, "invalid multinomial distribution (encountering probability entry < 0)");
-    PYGB_CHECK(code != W_ERR_INF, PYGB200_ERR_ARG, "invalid multinomial distribution (encountering probability entry = infinity or NaN)");
-    PYGB_CHECK(code != W_ERR_SUM, PYGB200_ERR_ARG, "invalid multinomial distribution (sum of probabilities <= 0)");
-    PYGB_CHECK(code != W_ERR_CATEGORIES, PYGB200_ERR_ARG, "number of categories cannot exceed 2^24");
-    return PYGB200_OK;
-  };
-  if (weighted && !s->wl_ready) {
-    if (int e = s->wl_tab.ensure(sizeof(kMklLogfTable), 0, st)) return e;
-    if (int e = s->wl_bits.ensure((size_t)1 << 21, 0, st)) return e;
-    PYGB_CUDA(cudaMemcpyAsync(s->wl_tab.p, kMklLogfTable, sizeof(kMklLogfTable), cudaMemcpyHostToDevice, st));
-    PYGB_CUDA(cudaMemsetAsync(s->wl_bits.p, 0, (size_t)1 << 21, st));
-    k_w_log_bitmap<<<ceil_div(kMklLogfTableN, NT), NT, 0, st>>>(s->wl_tab.as<u32>(), kMklLogfTableN, s->wl_bits.as<u32>());
-    PYGB_LAUNCH_CHECK();
-    s->wl_ready = true;
-  }
   // step 1: degrees -> per-node edge / engine-word / scratch offsets; the host reads the pass's totals (st_host)
-  auto biased_count = [&](const PassArgs& a, i64 F_grid, i64 E_prev) -> int {
-    const int g = std::max(grid_for(F_grid, NT, s->sm_count), a.lk_colv ? grid_for(E_prev, NT, s->sm_count) : 1);
-    void* tk = prof_begin(st);
-    if (idx32) launch_pdl(k_w_count<int32_t>, g, NT, 0, st, a); else launch_pdl(k_w_count<int64_t>, g, NT, 0, st, a);
-    prof_end(tk, "count", st, F_grid);
-    PYGB_LAUNCH_CHECK();
+  int biased_count(const PassArgs& a, i64 F_grid, i64 E_prev) {
+    if (int e = launch<PDL>("count", F_grid, k_w_count<idx_t>, count_grid(a, F_grid, E_prev), NT, 0, st, a)) return e;
     if (int e = read_state()) return e;
     return biased_error(s->st_host[ST_ERROR]);
-  };
+  }
   // step 2: size the key scratch and the raw stream from those totals, then draw: row / edge id / global dst id of every
   // sampled edge at its final position (what the schedules' insert stages start from)
-  auto biased_draws = [&](PassArgs& a, int r) -> int {
+  int biased_draws(PassArgs& a, int r) {
     const i64 F = s->st_host[ST_PASS_F], E = s->st_host[ST_PASS_E], W = s->st_host[ST_W_WORDS], S = s->st_host[ST_W_SCR];
     if (int e = s->wkey.ensure((size_t)std::max<i64>(S, 1) * 4, 0, st)) return e;
     if (int e = s->widx.ensure((size_t)std::max<i64>(S, 1) * 4, 0, st)) return e;
@@ -2155,160 +2257,111 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
     const i64 cap_need = need + 2 * (i64)s->jump_S + 8 * MT_N;
     if (cap_need > raw_cap) {
       PYGB_CHECK(cap_need < ((i64)1 << 33), PYGB200_ERR_UNSUPPORTED, "biased sampling: a run may consume at most 2^33 engine outputs");
-      i64 gen_now = 0;
-      PYGB_CUDA(cudaMemcpyAsync(&gen_now, s->gen.p, 8, cudaMemcpyDeviceToHost, st));
-      PYGB_CUDA(cudaStreamSynchronize(st));
-      if (int e = s->raw.ensure((size_t)cap_need * 4, (size_t)gen_now * 4, st)) return e;
-      raw_cap = s->raw_cap_words = (i64)(s->raw.cap / 4);
+      if (int e = grow_raw(cap_need)) return e;
     }
     void* tkm = prof_begin(st);
     if (int e = mt_request(s, st, need)) return e;
     prof_end(tkm, "mtgen", st, W);   // (raw mt19937 words of this pass: jump-ahead generation when there are many)
     a.raw = s->raw.as<u32>(); a.raw_cap = raw_cap;
     WArgs wa;
-    wa.weight = reinterpret_cast<const float*>(edge_weight[r]);
+    wa.weight = reinterpret_cast<const float*>(p.edge_weight[r]);
     wa.skey = s->wkey.as<float>(); wa.sidx = s->widx.as<u32>();
     wa.lbits = s->wl_bits.as<u32>(); wa.ltab = s->wl_tab.as<u32>(); wa.ltab_n = kMklLogfTableN;
     wa.wbase = out0 + eng_words + wwords;
     wwords += W;
-    void* tk = prof_begin(st);
     const int gw = (int)std::min<i64>(std::max<i64>(ceil_div(F, NT / 32), 1), (i64)s->sm_count * 16);
-    {
-      static const bool smem_ok = cudaFuncSetAttribute(k_w_sample<int32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, W_LIST_MAX * 2048) == cudaSuccess &&
-                                  cudaFuncSetAttribute(k_w_sample<int64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, W_LIST_MAX * 2048) == cudaSuccess;
-      PYGB_CHECK(smem_ok, PYGB200_ERR_CUDA, "k_w_sample: cannot reserve shared memory for the candidate lists");
-      const i64 kf = a.fanout;
-      const size_t smem = (!a.replace && kf >= 0 && kf + 1 <= W_LIST_MAX) ? (size_t)(kf + 1) * (NT / 32) * 32 * 8 : 0;
-      if (idx32) PYGB_CUDA(launch_pdl(k_w_sample<int32_t>, gw, NT, smem, st, a, wa));
-      else PYGB_CUDA(launch_pdl(k_w_sample<int64_t>, gw, NT, smem, st, a, wa));
-    }
-    prof_end(tk, "sample", st, E);
-    PYGB_LAUNCH_CHECK();
-    return PYGB200_OK;
-  };
+    static const bool smem_ok = cudaFuncSetAttribute(k_w_sample<idx_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, W_LIST_MAX * 2048) == cudaSuccess;
+    PYGB_CHECK(smem_ok, PYGB200_ERR_CUDA, "k_w_sample: cannot reserve shared memory for the candidate lists");
+    const i64 kf = a.fanout;
+    const size_t smem = (!a.replace && kf >= 0 && kf + 1 <= W_LIST_MAX) ? (size_t)(kf + 1) * (NT / 32) * 32 * 8 : 0;
+    return launch<PDL>("sample", E, k_w_sample<idx_t>, gw, NT, smem, st, a, wa);
+  }
   // v2 schedule: count -> draws -> inserts -> ids
-  auto biased_pass = [&](PassArgs& a, int r, i64 Fb) -> int {
+  int biased_pass(PassArgs& a, int r, i64 Fb) {
     if (int e = biased_count(a, Fb, 0)) return e;
     if (int e = biased_draws(a, r)) return e;
     const i64 Eg = std::max<i64>(s->st_host[ST_PASS_E], 1);
-    void* tk = prof_begin(st);
-    launch_pdl(k_v2_insert<false>, grid_for(Eg, 4 * NT, s->sm_count), NT, 0, st, a);
-    prof_end(tk, "insert", st, Eg);
-    PYGB_LAUNCH_CHECK();
+    if (int e = launch<PDL>("insert", Eg, k_v2_insert<false>, grid_for(Eg, 4 * NT, s->sm_count), NT, 0, st, a)) return e;
     return v2_ids(a, Eg);
-  };
+  }
 
   // ---- seeds (neighbor_kernel.cpp:409-416, :669-704)
-  if (any_time) if (int e = s->seed_times.ensure((size_t)std::max<i64>(total_seeds, 1) * 8, 0, st)) return e;
-  // The first pass that will run (hop 0) is counted inside the seed launch of its source type (extra blocks)
-  int fuse_r = -1, fuse_t = -1;
-  if (lat) {
-    for (int r = 0; r < R; ++r) {
-      if (num_neighbors[(size_t)r * L] == 0) continue;
-      if (fb[(size_t)rels[r].src_type * (L + 1)] == 0 || eb[(size_t)r * L] == 0) continue;
-      fuse_r = r; fuse_t = rels[r].src_type;
-      break;
+  int seeds() {
+    const int T = p.T, L = p.L;
+    const int64_t* n_seeds = p.n_seeds;
+    if (p.any_time) if (int e = s->seed_times.ensure((size_t)std::max<i64>(p.total_seeds, 1) * 8, 0, st)) return e;
+    i64 batch0 = 0;
+    for (int t = 0; t < T; batch0 += p.disjoint ? n_seeds[t] : 0, ++t) {
+      const idx_t* seed = (const idx_t*)p.seeds[t];
+      const i64 n = n_seeds[t];
+      PassArgs a = make_args(-1, t, -1);
+      a.seed_mode = 1;
+      PassArgs c = a;
+      int count_blocks = 0;
+      if (t == p.fuse_t) {
+        const int r = p.fuse_r;
+        c = make_args(p.rels[r].src_type, p.rels[r].dst_type, r);
+        c.fanout = p.k(r, 0);
+        count_blocks = (int)ceil_div(n, SEED_NT);
+      }
+      if (p.any_time && n > 0) {
+        const pygb200_temporal* temporal = p.temporal;
+        const i64* stt = temporal->seed_time ? reinterpret_cast<const i64*>(temporal->seed_time[t]) : nullptr;
+        const i64* ntt = temporal->node_time ? reinterpret_cast<const i64*>(temporal->node_time[t]) : nullptr;
+        if (int e = launch<PLAIN>(nullptr, 0, k_seed_times<idx_t>, grid_for(n, NT, s->sm_count), NT, 0, st, s->seed_times.as<i64>(), seed, n,
+                                  batch0, stt, ntt))
+          return e;
+      }
+      if (p.v2) {
+        if (n == 0) continue;   // the zeroed state already says "empty list, empty slice"
+        if (p.p2p) { a.pk_main = a.pk; a.pk_main_bits = a.pk_bits; a.pk = s->seedpk[s->v2_side].as<u64>(); a.pk_bits = s->seedpk_bits[s->v2_side]; }
+        a.sd_begin = lay.o_begin + t; a.sd_end = lay.o_end + t; a.sd_nph = lay.o_nph + t * (L + 1);   // (k_seed_end folded into the mark kernel)
+        if (int e = launch<PDL>("seed", n, k_v2_seed<idx_t>, grid_for(n, NT, s->sm_count), NT, 0, st, a, seed, n)) return e;
+        if (p.p2p) {
+          // seeds: every rank dedups ALL of them in a scratch table of its own (65 k CAS, L2-resident) — no exchange, no
+          // barrier; only the ids of the seeds a rank owns go into its partition of the real table (k_v2_assign)
+          if (int e = launch<PDL>("mark", n, k_v2_mark<true>, grid_for(n, ETILE, s->sm_count), NT, 0, st, a)) return e;
+          if (int e = launch<PDL>("assign", n, k_v2_assign<true>, grid_for(n, 4 * NT, s->sm_count), NT, 0, st, a)) return e;
+          // (the scratch table is wiped on the side stream with this side's table reset, behind the run)
+        } else if (int e = v2_ids(a, n)) return e;
+        continue;
+      }
+      if (n > 0 && n <= SEED_FUSED_MAX) {
+        if (int e = launch<PDL>(nullptr, 0, k_seed_fused<idx_t>, 1 + count_blocks, SEED_NT, 0, st, a, seed, (int)n, batch0, (int)L,
+                                lay.o_begin + t, lay.o_end + t, lay.o_nph + t * (L + 1), c))
+          return e;
+      } else if (n > 0) {
+        const int g = grid_for(n, NT, s->sm_count);
+        if (int e = launch<PLAIN>(nullptr, 0, k_seed<idx_t>, g, NT, 0, st, a, seed, n, batch0)) return e;
+        if (int e = launch<PDL>(nullptr, 0, k_mark, grid_for(n, ETILE, s->sm_count), NT, 0, st, a)) return e;
+        if (int e = launch<PDL>(nullptr, 0, k_assign, g, NT, 0, st, a)) return e;
+        if (int e = launch<PLAIN>(nullptr, 0, k_seed_end, 1, 1, 0, st, dst, t, L, lay.o_list, lay.o_begin, lay.o_end, lay.o_nph)) return e;
+      }  // n == 0: the zeroed state already says "empty list, empty slice"
     }
-  }
-  std::vector<i64> batch_base((size_t)T, 0);
-  if (disjoint) for (int t = 1; t < T; ++t) batch_base[t] = batch_base[t - 1] + n_seeds[t - 1];
-  for (int t = 0; t < T; ++t) {
-    const i64 batch0 = batch_base[t];
-    PassArgs a = make_args(-1, t, -1);
-    a.seed_mode = 1;
-    PassArgs c = a;
-    int count_blocks = 0;
-    if (t == fuse_t) {
-      c = make_args(rels[fuse_r].src_type, rels[fuse_r].dst_type, fuse_r);
-      c.fanout = num_neighbors[(size_t)fuse_r * L];
-      count_blocks = (int)ceil_div(n_seeds[t], SEED_NT);
-    }
-    if (any_time && n_seeds[t] > 0) {
-      const i64* stt = temporal->seed_time ? reinterpret_cast<const i64*>(temporal->seed_time[t]) : nullptr;
-      const i64* ntt = temporal->node_time ? reinterpret_cast<const i64*>(temporal->node_time[t]) : nullptr;
-      const int g = grid_for(n_seeds[t], NT, s->sm_count);
-      if (idx32) k_seed_times<int32_t><<<g, NT, 0, st>>>(s->seed_times.as<i64>(), (const int32_t*)seeds[t], n_seeds[t], batch0, stt, ntt);
-      else k_seed_times<int64_t><<<g, NT, 0, st>>>(s->seed_times.as<i64>(), (const int64_t*)seeds[t], n_seeds[t], batch0, stt, ntt);
-      PYGB_LAUNCH_CHECK();
-    }
-    if (v2) {
-      if (n_seeds[t] == 0) continue;   // the zeroed state already says "empty list, empty slice"
-      if (p2p) { a.pk_main = a.pk; a.pk_main_bits = a.pk_bits; a.pk = s->seedpk[s->v2_side].as<u64>(); a.pk_bits = s->seedpk_bits[s->v2_side]; }
-      a.sd_begin = lay.o_begin + t; a.sd_end = lay.o_end + t; a.sd_nph = lay.o_nph + t * (L + 1);   // (k_seed_end folded into the mark kernel)
-      const int g = grid_for(n_seeds[t], NT, s->sm_count);
-      void* tks = prof_begin(st);
-      if (idx32) launch_pdl(k_v2_seed<int32_t>, g, NT, 0, st, a, (const int32_t*)seeds[t], (i64)n_seeds[t]);
-      else launch_pdl(k_v2_seed<int64_t>, g, NT, 0, st, a, (const int64_t*)seeds[t], (i64)n_seeds[t]);
-      prof_end(tks, "seed", st, n_seeds[t]);
-      PYGB_LAUNCH_CHECK();
-      if (p2p) {
-        // seeds: every rank dedups ALL of them in a scratch table of its own (65 k CAS, L2-resident) — no exchange, no
-        // barrier; only the ids of the seeds a rank owns go into its partition of the real table (k_v2_assign)
-        tks = prof_begin(st);
-        launch_pdl(k_v2_mark<true>, grid_for(n_seeds[t], ETILE, s->sm_count), NT, 0, st, a);
-        prof_end(tks, "mark", st, n_seeds[t]);
-        PYGB_LAUNCH_CHECK();
-        tks = prof_begin(st);
-        launch_pdl(k_v2_assign<true>, grid_for(n_seeds[t], 4 * NT, s->sm_count), NT, 0, st, a);
-        prof_end(tks, "assign", st, n_seeds[t]);
-        PYGB_LAUNCH_CHECK();
-        // (the scratch table is wiped on the side stream with this side's table reset, behind the run)
-      } else if (int e = v2_ids(a, n_seeds[t])) return e;
-      continue;
-    }
-    if (n_seeds[t] > 0 && n_seeds[t] <= SEED_FUSED_MAX) {
-      if (idx32) launch_pdl(k_seed_fused<int32_t>, 1 + count_blocks, SEED_NT, 0, st, a, (const int32_t*)seeds[t], (int)n_seeds[t], batch0, (int)L,
-                            lay.o_begin + t, lay.o_end + t, lay.o_nph + t * (L + 1), c);
-      else launch_pdl(k_seed_fused<int64_t>, 1 + count_blocks, SEED_NT, 0, st, a, (const int64_t*)seeds[t], (int)n_seeds[t], batch0, (int)L,
-                      lay.o_begin + t, lay.o_end + t, lay.o_nph + t * (L + 1), c);
-      PYGB_LAUNCH_CHECK();
-    } else if (n_seeds[t] > 0) {
-      const int g = grid_for(n_seeds[t], NT, s->sm_count);
-      if (idx32) k_seed<int32_t><<<g, NT, 0, st>>>(a, (const int32_t*)seeds[t], n_seeds[t], batch0);
-      else k_seed<int64_t><<<g, NT, 0, st>>>(a, (const int64_t*)seeds[t], n_seeds[t], batch0);
-      PYGB_LAUNCH_CHECK();
-      launch_pdl(k_mark, grid_for(n_seeds[t], ETILE, s->sm_count), NT, 0, st, a);
-      PYGB_LAUNCH_CHECK();
-      launch_pdl(k_assign, g, NT, 0, st, a);
-      PYGB_LAUNCH_CHECK();
-      k_seed_end<<<1, 1, 0, st>>>(dst, t, L, lay.o_list, lay.o_begin, lay.o_end, lay.o_nph);
-      PYGB_LAUNCH_CHECK();
-    }  // n == 0: the zeroed state already says "empty list, empty slice"
+    return PYGB200_OK;
   }
 
-  // ---- hops.  Bounded mode defers every pass's lookup into the next k_count / the final kernel.
-  i64* lk_colv = nullptr; const u64* lk_vals = nullptr; i64 lk_E = 0;
-  s->run_serial += 1;
-  bool published = false;
-  int pub_w_list = -1;   // latency path: the counter that arrives as the flag word's payload
-  // latency path: the static schedule decides which write-once word holds what
-  struct Wd { int w; i64 c; };
-  std::vector<Wd> cur_list, sl_begin, sl_end, relcum, list_end;
-  std::vector<int> eph_w;
-  Wd cursor{-1, 0};
-  int lk_w_E = -1, lk_w_pbase = -1;
-  if (lat) {
+  // ---- hops, latency schedule: every pass's counters are write-once words fixed here, no host synchronisation
+  int hops_latency() {
+    const int T = p.T, R = p.R, L = p.L;
     cur_list.resize(T); sl_begin.resize(T); sl_end.resize(T); relcum.assign(R, Wd{-1, 0});
     list_end.resize((size_t)T * (L + 1)); eph_w.assign((size_t)R * L, -1);
     for (int t = 0; t < T; ++t) {
-      cur_list[t] = Wd{-1, n_seeds[t]}; sl_begin[t] = Wd{-1, 0}; sl_end[t] = Wd{-1, n_seeds[t]};
+      cur_list[t] = Wd{-1, p.n_seeds[t]}; sl_begin[t] = Wd{-1, 0}; sl_end[t] = Wd{-1, p.n_seeds[t]};
       list_end[(size_t)t * (L + 1)] = cur_list[t];
     }
     int P = 0, P_total = 0;
     for (int h = 0; h < L; ++h)
-      for (int r = 0; r < R; ++r)
-        P_total += num_neighbors[(size_t)r * L + h] != 0 && fb[(size_t)rels[r].src_type * (L + 1) + h] != 0 && eb[(size_t)r * L + h] != 0;
+      for (int r = 0; r < R; ++r) P_total += p.launches(r, h);
     for (int h = 0; h < L; ++h) {
       for (int r = 0; r < R; ++r) {
-        const i64 k = num_neighbors[(size_t)r * L + h];
-        const int src_t = rels[r].src_type, dst_t = rels[r].dst_type;
-        if (k == 0) continue;  // nothing emitted, no RNG consumed (neighbor_kernel.cpp:67-68)
-        const i64 Fb = fb[(size_t)src_t * (L + 1) + h], Eb = eb[(size_t)r * L + h];
-        if (Fb == 0 || Eb == 0) continue;
+        // k == 0: nothing emitted, no RNG consumed (neighbor_kernel.cpp:67-68)
+        if (!p.launches(r, h)) continue;
+        const i64 k = p.k(r, h), Fb = p.F(r, h), Eb = p.E(r, h);
+        const int src_t = p.rels[r].src_type, dst_t = p.rels[r].dst_type;
         PassArgs a = make_args(src_t, dst_t, r);
         if (P == P_total - 1) {   // the last pass publishes the run from its k_assign_s
-          a.pub_host = s->st_host_dev; a.pub_zero = dst_other; a.pub_serial = s->run_serial; a.pub_words = (int)lay.words;
-          a.pub_o_mt = lay.o_mt;
+          publish(a);
           published = true;
         }
         const int base = lay.o_ssa + 5 * P++;
@@ -2323,28 +2376,13 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
         if (a.pub_words) pub_w_list = base + 3;
         a.w_seed_list = lay.o_list + dst_t; a.w_seed_ids = lay.o_ids + dst_t;
         a.lk_colv = lk_colv; a.lk_vals = lk_vals; a.lk_w_E = lk_w_E; a.lk_w_pbase = lk_w_pbase;
-        void* tk;
-        if (!(h == 0 && r == fuse_r)) {   // (else: counted inside the seed launch)
-          const int g = std::max(grid_for(Fb, NT, s->sm_count), lk_colv ? grid_for(lk_E, NT, s->sm_count) : 1);
-          tk = prof_begin(st);
-          if (idx32) launch_pdl(k_count_s<int32_t>, g, NT, 0, st, a); else launch_pdl(k_count_s<int64_t>, g, NT, 0, st, a);
-          prof_end(tk, "count", st, Fb);
-          PYGB_LAUNCH_CHECK();
-        }
+        if (!(h == 0 && r == p.fuse_r))   // (else: counted inside the seed launch)
+          if (int e = launch<PDL>("count", Fb, k_count_s<idx_t>, count_grid(a, Fb, lk_E), NT, 0, st, a)) return e;
         a.group = sample_group_lanes(k);
         const int gs = grid_for(Fb, sample_nodes_per_block(a.group), s->sm_count);
-        tk = prof_begin(st);
-        if (idx32) launch_pdl(k_sample_s<int32_t>, gs, NT, 0, st, a); else launch_pdl(k_sample_s<int64_t>, gs, NT, 0, st, a);
-        prof_end(tk, "sample", st, Eb);
-        PYGB_LAUNCH_CHECK();
-        tk = prof_begin(st);
-        launch_pdl(k_mark_s, grid_for(Eb, ETILE, s->sm_count), NT, 0, st, a);
-        prof_end(tk, "mark", st, Eb);
-        PYGB_LAUNCH_CHECK();
-        tk = prof_begin(st);
-        launch_pdl(k_assign_s, grid_for(Eb, NT, s->sm_count), NT, 0, st, a);
-        prof_end(tk, "assign", st, Eb);
-        PYGB_LAUNCH_CHECK();
+        if (int e = launch<PDL>("sample", Eb, k_sample_s<idx_t>, gs, NT, 0, st, a)) return e;
+        if (int e = launch<PDL>("mark", Eb, k_mark_s, grid_for(Eb, ETILE, s->sm_count), NT, 0, st, a)) return e;
+        if (int e = launch<PDL>("assign", Eb, k_assign_s, grid_for(Eb, NT, s->sm_count), NT, 0, st, a)) return e;
         lk_colv = a.colv; lk_vals = a.vals; lk_E = Eb; lk_w_E = base; lk_w_pbase = relcum[r].w;
         cursor = Wd{base + 1, 0}; relcum[r] = Wd{base + 2, 0}; cur_list[dst_t] = Wd{base + 3, 0};
         eph_w[(size_t)r * L + h] = base;
@@ -2354,156 +2392,131 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
         list_end[(size_t)t * (L + 1) + h + 1] = cur_list[t];
       }
     }
+    return PYGB200_OK;
   }
-  for (int h = 0; h < L && !lat; ++h) {
-    if (synced) if (int e = read_state()) return e;  // actual frontier slices of this hop
-    // last pass of this hop that will actually be launched (it also does the end-of-hop bookkeeping)
-    int last_r = -1;
-    for (int r = 0; r < R; ++r) {
-      const i64 k = num_neighbors[(size_t)r * L + h];
-      if (k == 0) continue;
-      if (!synced && (fb[(size_t)rels[r].src_type * (L + 1) + h] == 0 || eb[(size_t)r * L + h] == 0)) continue;
-      if (synced && s->st_host[lay.o_end + rels[r].src_type] - s->st_host[lay.o_begin + rels[r].src_type] == 0) continue;
-      last_r = r;
-    }
-    bool hop_closed = false;
-    for (int r = 0; r < R; ++r) {
-      const i64 k = num_neighbors[(size_t)r * L + h];
-      const int src_t = rels[r].src_type, dst_t = rels[r].dst_type;
-      if (k == 0) continue;  // nothing emitted, no RNG consumed (neighbor_kernel.cpp:67-68)
-      auto with_hop_end = [&](PassArgs& a) {
-        if (r != last_r) return;
-        a.he_T = T; a.he_L = L; a.he_hop = h; a.he_list = lay.o_list; a.he_begin = lay.o_begin; a.he_end = lay.o_end;
-        a.he_nph = lay.o_nph;
-      };
-      if (!synced) {
-        const i64 Fb = fb[(size_t)src_t * (L + 1) + h], Eb = eb[(size_t)r * L + h];
-        if (Fb == 0 || Eb == 0) continue;
-        PassArgs a = make_args(src_t, dst_t, r);
-        a.fanout = k;
-        a.o_eph = lay.o_eph + r * L + h;
+
+  // ---- hops, bounded (v2 and wide-table) runs: buffers are sized from the static bounds, every pass's lookup is deferred
+  // into the next k_count / the final kernel
+  int hops_bounded() {
+    const int R = p.R, L = p.L;
+    for (int h = 0; h < L; ++h) {
+      int last_r = -1;   // last pass of this hop that will actually be launched (it also does the end-of-hop bookkeeping)
+      for (int r = 0; r < R; ++r) if (p.launches(r, h)) last_r = r;
+      bool hop_closed = false;
+      for (int r = 0; r < R; ++r) {
+        // k == 0: nothing emitted, no RNG consumed (neighbor_kernel.cpp:67-68)
+        if (!p.launches(r, h)) continue;
+        const i64 Fb = p.F(r, h), Eb = p.E(r, h);
+        PassArgs a = pass_args(r, h);
         a.lk_colv = lk_colv; a.lk_vals = lk_vals;
-        with_hop_end(a);
-        if (!wrel[r]) if (int e = idx32 ? launch_count<int32_t>(s, a, Fb, lk_E, st) : launch_count<int64_t>(s, a, Fb, lk_E, st)) return e;
-        if (v2) {
-          // does any later pass insert into this dst type's table?  (else the ids need not be written back)
-          a.v2_writeback = 0;
-          for (int h2 = h; h2 < L && !a.v2_writeback; ++h2)
-            for (int r2 = (h2 == h ? r + 1 : 0); r2 < R && !a.v2_writeback; ++r2)
-              a.v2_writeback = rels[r2].dst_type == dst_t && num_neighbors[(size_t)r2 * L + h2] != 0 &&
-                               fb[(size_t)rels[r2].src_type * (L + 1) + h2] != 0 && eb[(size_t)r2 * L + h2] != 0;
-          if (wrel[r]) {
-            if (int e = biased_pass(a, r, Fb)) return e;
-            if (r == last_r) hop_closed = true;
-            continue;
-          }
-          a.group = sample_group_lanes(k);
-          const int gs = grid_for(p2p ? ceil_div(Fb, XW) + 1 : Fb, sample_nodes_per_block(a.group), s->sm_count);
-          void* tk = prof_begin(st);
-          if (p2p) {
-            // (the positions of the ranks' frontier slices were written by the last block of k_count)
-            if (idx32) launch_pdl(k_v2_sample<int32_t, true>, gs, NT, 0, st, a); else launch_pdl(k_v2_sample<int64_t, true>, gs, NT, 0, st, a);
-            prof_end(tk, "sample", st, Eb);
-            PYGB_LAUNCH_CHECK();
-            // own slice -> every peer with 16-byte stores; its last block raises this rank's flag at the peers ("my slice
-            // has been delivered"), so the peers' flags arrive while the rows are written and k_v2_insert only has to look
-            a.x_timeout_ns = xbar_timeout_ns;
-            a.x_sig_epoch = ++s->x.epoch;
-            tk = prof_begin(st);
-            launch_pdl(k_v2_push, grid_for(ceil_div(Eb, XW) + 1, 4 * NT, s->sm_count), NT, 0, st, a);
-            prof_end(tk, "push", st, Eb);
-            PYGB_LAUNCH_CHECK();
-            a.x_sig_epoch = 0;
-            tk = prof_begin(st);
-            launch_pdl(k_v2_rows, grid_for(Fb, NT, s->sm_count), NT, 0, st, a);
-            prof_end(tk, "rows", st, Eb);
-            PYGB_LAUNCH_CHECK();
-          } else {
-            // draws and table inserts in one kernel
-            if (idx32) launch_pdl(k_v2_sample<int32_t, false>, gs, NT, 0, st, a); else launch_pdl(k_v2_sample<int64_t, false>, gs, NT, 0, st, a);
-            prof_end(tk, "sample", st, Eb);
-            PYGB_LAUNCH_CHECK();
-          }
-          if (p2p) {
-            if (int e = xbarrier(a)) return e;   // until everybody's (dst, edge id) have arrived
-            void* tki = prof_begin(st);
-            launch_pdl(k_v2_insert<true>, grid_for(Eb, 4 * NT, s->sm_count), NT, 0, st, a);
-            prof_end(tki, "insert", st, Eb);
-            PYGB_LAUNCH_CHECK();
-          }
-          if (int e = v2_ids(a, Eb)) return e;
-          if (p2p) s->x.passes += 1;
-          if (r == last_r) hop_closed = true;
-          continue;
-        }
-        if (wrel[r]) {   // wide table (disjoint / 64-bit ids): biased draws, then the expand-from-edge-ids stage the sharded path uses
+        if (r == last_r) with_hop_end(a, h);
+        if (!p.wrel[r]) if (int e = count(a, Fb, lk_E)) return e;
+        if (p.v2) {
+          if (int e = pass_v2(a, r, h)) return e;
+        } else if (p.wrel[r]) {   // wide table (disjoint / 64-bit ids): biased draws, then the expand-from-edge-ids stage the sharded path uses
           if (int e = biased_count(a, Fb, lk_E)) return e;
           if (int e = biased_draws(a, r)) return e;
-          if (nodedup) continue;   // (row / edge id / global id are already what a distributed hop returns)
-          PassArgs d = a;
-          d.phase = 2;
-          if (int e = idx32 ? launch_sample<int32_t>(s, d, Fb, Eb, st) : launch_sample<int64_t>(s, d, Fb, Eb, st)) return e;
-          if (int e = idx32 ? launch_rest<int32_t>(s, a, Fb, Eb, false, st, false) : launch_rest<int64_t>(s, a, Fb, Eb, false, st, false)) return e;
+          if (p.nodedup) continue;   // (row / edge id / global id are already what a distributed hop returns)
+          if (int e = expand(a, Fb, Eb, false)) return e;
           lk_colv = a.colv; lk_vals = a.vals; lk_E = Eb;
-          if (r == last_r) hop_closed = true;
-          continue;
-        }
-        if (nodedup) {   // draw + gather only: global ids stay in `colv`, nothing is mapped, no lookup follows
+        } else if (p.nodedup) {   // draw + gather only: global ids stay in `colv`, nothing is mapped, no lookup follows
           PassArgs d = a;
           d.phase = 3;
-          if (int e = idx32 ? launch_sample<int32_t>(s, d, Fb, Eb, st) : launch_sample<int64_t>(s, d, Fb, Eb, st)) return e;
+          if (int e = sample(d, Fb, Eb)) return e;
           continue;
-        }
-        if (!sharded) {
-          if (int e = idx32 ? launch_rest<int32_t>(s, a, Fb, Eb, false, st) : launch_rest<int64_t>(s, a, Fb, Eb, false, st)) return e;
         } else {
-          // every rank counted the whole frontier (offsets and bit-stream positions are global); draw only
-          // this rank's slice, all-gather the edge ids, then expand/dedup everything (replicated)
-          const int W = shard->world;
-          k_shard_bounds<<<1, 128, 0, st>>>(a, W, lay.o_shard);
-          PYGB_LAUNCH_CHECK();
-          if (int e = read_state()) return e;
-          const i64 F = s->st_host[ST_PASS_F], E = s->st_host[ST_PASS_E], pbase = s->st_host[ST_PASS_BASE];
-          PassArgs d = a;
-          d.phase = 1;
-          d.shard_lo = (i64)((__int128)F * shard->rank / W);
-          d.shard_hi = (i64)((__int128)F * (shard->rank + 1) / W);
-          if (d.shard_hi > d.shard_lo)
-            if (int e = idx32 ? launch_sample<int32_t>(s, d, d.shard_hi - d.shard_lo, E, st) : launch_sample<int64_t>(s, d, d.shard_hi - d.shard_lo, E, st)) return e;
-          if (E > 0) {
-            const int rc = shard->allgather(shard->user, a.eid + pbase, reinterpret_cast<const int64_t*>(s->st_host + lay.o_shard), W, (void*)st);
-            PYGB_CHECK(rc == 0, PYGB200_ERR_INTERNAL, "frontier-sharded sampling: all-gather callback failed");
-          }
-          d.phase = 2;
-          if (int e = idx32 ? launch_sample<int32_t>(s, d, Fb, Eb, st) : launch_sample<int64_t>(s, d, Fb, Eb, st)) return e;
-          if (int e = idx32 ? launch_rest<int32_t>(s, a, Fb, Eb, false, st, false) : launch_rest<int64_t>(s, a, Fb, Eb, false, st, false)) return e;
+          if (int e = p.sharded ? pass_collective(a, Fb, Eb) : rest(a, Fb, Eb, false)) return e;
+          lk_colv = a.colv; lk_vals = a.vals; lk_E = Eb;
         }
-        lk_colv = a.colv; lk_vals = a.vals; lk_E = Eb;
         if (r == last_r) hop_closed = true;
-      } else {
-        const i64 F = s->st_host[lay.o_end + src_t] - s->st_host[lay.o_begin + src_t];
+      }
+      if (!hop_closed) if (int e = hop_end(h)) return e;
+    }
+    return PYGB200_OK;
+  }
+  // v2 pass after its count (a biased one counts itself): draws, inserts, ids
+  int pass_v2(PassArgs& a, int r, int h) {
+    const int R = p.R, L = p.L, dst_t = p.rels[r].dst_type;
+    const i64 Fb = p.F(r, h), Eb = p.E(r, h);
+    // does any later pass insert into this dst type's table?  (else the ids need not be written back)
+    a.v2_writeback = 0;
+    for (int h2 = h; h2 < L && !a.v2_writeback; ++h2)
+      for (int r2 = (h2 == h ? r + 1 : 0); r2 < R && !a.v2_writeback; ++r2)
+        a.v2_writeback = p.rels[r2].dst_type == dst_t && p.launches(r2, h2);
+    if (p.wrel[r]) return biased_pass(a, r, Fb);
+    a.group = sample_group_lanes(a.fanout);
+    const int gs = grid_for(p.p2p ? ceil_div(Fb, p.XW) + 1 : Fb, sample_nodes_per_block(a.group), s->sm_count);
+    if (!p.p2p) {   // draws and table inserts in one kernel
+      if (int e = launch<PDL>("sample", Eb, k_v2_sample<idx_t, false>, gs, NT, 0, st, a)) return e;
+      return v2_ids(a, Eb);
+    }
+    // (the positions of the ranks' frontier slices were written by the last block of k_count)
+    if (int e = launch<PDL>("sample", Eb, k_v2_sample<idx_t, true>, gs, NT, 0, st, a)) return e;
+    // own slice -> every peer with 16-byte stores; its last block raises this rank's flag at the peers ("my slice
+    // has been delivered"), so the peers' flags arrive while the rows are written and k_v2_insert only has to look
+    a.x_timeout_ns = xbar_timeout_ns();
+    a.x_sig_epoch = ++s->x.epoch;
+    if (int e = launch<PDL>("push", Eb, k_v2_push, grid_for(ceil_div(Eb, p.XW) + 1, 4 * NT, s->sm_count), NT, 0, st, a)) return e;
+    a.x_sig_epoch = 0;
+    if (int e = launch<PDL>("rows", Eb, k_v2_rows, grid_for(Fb, NT, s->sm_count), NT, 0, st, a)) return e;
+    if (int e = xbarrier(a)) return e;   // until everybody's (dst, edge id) have arrived
+    if (int e = launch<PDL>("insert", Eb, k_v2_insert<true>, grid_for(Eb, 4 * NT, s->sm_count), NT, 0, st, a)) return e;
+    if (int e = v2_ids(a, Eb)) return e;
+    s->x.passes += 1;
+    return PYGB200_OK;
+  }
+  // collective frontier sharding, after the count: every rank counted the whole frontier (offsets and bit-stream positions
+  // are global); draw only this rank's slice, all-gather the edge ids, then expand/dedup everything (replicated)
+  int pass_collective(const PassArgs& a, i64 Fb, i64 Eb) {
+    const pygb200_shard* shard = p.shard;
+    const int W = shard->world;
+    if (int e = launch<PLAIN>(nullptr, 0, k_shard_bounds, 1, 128, 0, st, a, W, lay.o_shard)) return e;
+    if (int e = read_state()) return e;
+    const i64 F = s->st_host[ST_PASS_F], E = s->st_host[ST_PASS_E], pbase = s->st_host[ST_PASS_BASE];
+    PassArgs d = a;
+    d.phase = 1;
+    d.shard_lo = (i64)((__int128)F * shard->rank / W);
+    d.shard_hi = (i64)((__int128)F * (shard->rank + 1) / W);
+    if (d.shard_hi > d.shard_lo) if (int e = sample(d, d.shard_hi - d.shard_lo, E)) return e;
+    if (E > 0) {
+      const int rc = shard->allgather(shard->user, a.eid + pbase, reinterpret_cast<const int64_t*>(s->st_host + lay.o_shard), W, (void*)st);
+      PYGB_CHECK(rc == 0, PYGB200_ERR_INTERNAL, "frontier-sharded sampling: all-gather callback failed");
+    }
+    return expand(a, Fb, Eb, false);
+  }
+
+  // ---- hops, host-synced runs (-1 fan-outs, > 8 GiB worst case, mixed biased / uniform relations): the host reads every
+  // hop's frontier and every pass's count, and sizes the buffers from the actual numbers
+  int hops_synced() {
+    const int R = p.R, L = p.L;
+    const i64* hs = s->st_host;
+    for (int h = 0; h < L; ++h) {
+      if (int e = read_state()) return e;  // actual frontier slices of this hop
+      auto frontier = [&](int r) { return hs[lay.o_end + p.rels[r].src_type] - hs[lay.o_begin + p.rels[r].src_type]; };
+      int last_r = -1;   // last pass of this hop that will actually be launched (it also does the end-of-hop bookkeeping)
+      for (int r = 0; r < R; ++r) if (p.k(r, h) != 0 && frontier(r) != 0) last_r = r;
+      bool hop_closed = false;
+      for (int r = 0; r < R; ++r) {
+        const i64 k = p.k(r, h);
+        const int dst_t = p.rels[r].dst_type;
+        const bool wrel = p.wrel[r];
+        if (k == 0) continue;  // nothing emitted, no RNG consumed (neighbor_kernel.cpp:67-68)
+        const i64 F = frontier(r);
         if (F == 0) continue;
         if (int e = ensure_frontier_scratch(s, F, st)) return e;
-        i64 eng_blocks = 0;   // mixed: blocks of the RandintEngine this pass may touch
-        if (k > 0 && !wrel[r]) {  // draws possible: make sure the raw stream buffer can hold this pass
-          const i64 upu = rels[r].num_edges < 65536 ? 1 : (rels[r].num_edges < ((i64)1 << 32) ? 3 : 7);
+        if (k > 0 && !wrel) {  // draws possible: make sure the raw stream buffer can hold this pass
+          const i64 upu = p.rels[r].num_edges < 65536 ? 1 : (p.rels[r].num_edges < ((i64)1 << 32) ? 3 : 7);
           if (int e = read_state()) return e;
-          eng_blocks = rng_blocks_for_units(s->st_host[ST_CURSOR] + sat_mul(sat_mul(F, k), upu)) + 1;
-          const i64 need = out0 + 256 * eng_blocks + wwords + 3 * MT_N + (mixed ? 2 * (i64)s->jump_S + 8 * MT_N : 0);
-          if (need > raw_cap) {
-            i64 gen_now = 0;
-            PYGB_CUDA(cudaMemcpyAsync(&gen_now, s->gen.p, 8, cudaMemcpyDeviceToHost, st));
-            PYGB_CUDA(cudaStreamSynchronize(st));
-            if (int e = s->raw.ensure((size_t)need * 4, (size_t)gen_now * 4, st)) return e;
-            raw_cap = s->raw_cap_words = (i64)(s->raw.cap / 4);
-          }
-          if (mixed) {
+          const i64 eng_blocks = rng_blocks_for_units(hs[ST_CURSOR] + sat_mul(sat_mul(F, k), upu)) + 1;   // engine blocks this pass may touch
+          const i64 need = out0 + 256 * eng_blocks + wwords + 3 * MT_N + (p.mixed ? 2 * (i64)s->jump_S + 8 * MT_N : 0);
+          if (need > raw_cap) if (int e = grow_raw(need)) return e;
+          if (p.mixed) {
             // ---- mixed biased / uniform relations.  The reference's RandintEngine fetches a block of 256 engine outputs whenever it
             // runs out (rand_engine.h:53-61,80-85); biased relations take outputs in between, so block b of the engine sits at
             // out0 + 256 b + (outputs the biased passes had consumed when b was fetched).  The uniform kernels index a stream in
             // which the blocks are contiguous: that stream is kept as a compacted copy (`eraw`).  Blocks the engine has already
             // fetched (b < used) stay; every block it may fetch during this pass is (re)copied from where it would sit NOW.
-            const i64 used = rng_blocks_for_units(s->st_host[ST_CURSOR]);
+            const i64 used = rng_blocks_for_units(hs[ST_CURSOR]);
             if (int e = mt_request(s, st, out0 + 256 * eng_blocks + wwords + 2 * MT_N)) return e;
             if (int e = s->eraw.ensure((size_t)eng_blocks * 256 * 4, (size_t)used * 256 * 4, st)) return e;
             PYGB_CUDA(cudaMemcpyAsync(s->eraw.as<u32>() + 256 * used, s->raw.as<u32>() + out0 + 256 * used + wwords,
@@ -2511,94 +2524,122 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
             eng_blocks_max = std::max(eng_blocks_max, eng_blocks);
           }
         }
-        PassArgs a = make_args(src_t, dst_t, r);
-        a.fanout = k;
-        a.o_eph = lay.o_eph + r * L + h;
-        auto use_eraw = [&](PassArgs& x) { if (mixed && !wrel[r]) { x.raw = s->eraw.as<u32>(); x.out0 = 0; x.raw_cap = (i64)(s->eraw.cap / 4); } };
-        use_eraw(a);
-        if (wrel[r]) {
+        PassArgs a = pass_args(r, h);
+        if (wrel) {
           if (int e = biased_count(a, F, 0)) return e;
         } else {
-          if (int e = idx32 ? launch_count<int32_t>(s, a, F, 0, st) : launch_count<int64_t>(s, a, F, 0, st)) return e;
+          if (int e = count(a, F, 0)) return e;
           if (int e = read_state()) return e;
         }
-        const i64 E = s->st_host[ST_PASS_E];
+        const i64 E = hs[ST_PASS_E];
         if (E == 0) continue;  // (a hop whose last pass emits nothing is closed by the standalone kernel below)
-        const i64 rel_before = s->st_host[ST_PASS_BASE], list_now = s->st_host[lay.o_list + dst_t];
+        const i64 rel_before = hs[ST_PASS_BASE], list_now = hs[lay.o_list + dst_t];
         if (int e = ensure_rel(s, r, rel_before + E, rel_before, st)) return e;
         if (int e = ensure_edge_scratch(s, E, st)) return e;
-        if (int e = ensure_type(s, dst_t, list_now + E, list_now, disjoint, st)) return e;
+        if (int e = ensure_type(s, dst_t, list_now + E, list_now, p.disjoint, st)) return e;
         if (int e = ensure_table(s, dst_t, list_now + E, list_now, st)) return e;
-        a = make_args(src_t, dst_t, r);  // pointers may have moved
-        a.fanout = k;
-        a.o_eph = lay.o_eph + r * L + h;
-        use_eraw(a);
-        if (wrel[r]) if (int e = biased_draws(a, r)) return e;   // (row / edge id / global dst id of every sampled edge)
-        if (nodedup) {
-          if (wrel[r]) continue;
+        a = pass_args(r, h);  // pointers may have moved
+        if (wrel) if (int e = biased_draws(a, r)) return e;   // (row / edge id / global dst id of every sampled edge)
+        if (p.nodedup) {
+          if (wrel) continue;
           a.phase = 3;
-          if (int e = idx32 ? launch_sample<int32_t>(s, a, F, E, st) : launch_sample<int64_t>(s, a, F, E, st)) return e;
+          if (int e = sample(a, F, E)) return e;
           continue;
         }
-        with_hop_end(a);
-        if (wrel[r]) {
-          PassArgs d = a;
-          d.phase = 2;   // expand from the edge ids: gather, hash insert
-          if (int e = idx32 ? launch_sample<int32_t>(s, d, F, E, st) : launch_sample<int64_t>(s, d, F, E, st)) return e;
-          if (int e = idx32 ? launch_rest<int32_t>(s, a, F, E, true, st, false) : launch_rest<int64_t>(s, a, F, E, true, st, false)) return e;
-        } else if (int e = idx32 ? launch_rest<int32_t>(s, a, F, E, true, st) : launch_rest<int64_t>(s, a, F, E, true, st)) return e;
+        if (r == last_r) with_hop_end(a, h);
+        if (int e = wrel ? expand(a, F, E, true) : rest(a, F, E, true)) return e;
         if (r == last_r) hop_closed = true;
       }
+      if (!hop_closed) if (int e = hop_end(h)) return e;
     }
-    if (!hop_closed) {
-      k_hop_end<<<1, 1024, 0, st>>>(dst, T, L, h, lay.o_list, lay.o_begin, lay.o_end, lay.o_nph);
-      PYGB_LAUNCH_CHECK();
-    }
+    return PYGB200_OK;
   }
 
-  if (mixed) if (int e = mt_request(s, st, out0 + 256 * eng_blocks_max + wwords + 2 * MT_N)) return e;   // (the state k_final publishes)
-  // ---- final kernel (deferred lookup of the last pass + engine state), counts to the host
-  {
-    PassArgs a = make_args(-1, 0, -1);
-    a.lk_colv = lk_colv; a.lk_vals = lk_vals;
-    if (lat) { a.ssa = 1; a.lk_w_E = lk_w_E; a.lk_w_pbase = lk_w_pbase; a.w_cur_in = cursor.w; }
-    if (!published) {
-      a.pub_host = s->st_host_dev; a.pub_zero = dst_other; a.pub_serial = s->run_serial; a.pub_words = (int)lay.words;
-      a.pub_o_mt = lay.o_mt;
+  // ---- final kernel (deferred lookup of the last pass + engine state), table cleanup, the wait for the run, results
+  int finish(pygb200_mt19937* mt, int64_t* nodes_per_hop, int64_t* edges_per_hop, int64_t* n_nodes_out, int64_t* n_edges_out) {
+    const int T = p.T;
+    if (p.mixed) if (int e = mt_request(s, st, out0 + 256 * eng_blocks_max + wwords + 2 * MT_N)) return e;   // (the state k_final publishes)
+    {
+      PassArgs a = make_args(-1, 0, -1);
+      a.lk_colv = lk_colv; a.lk_vals = lk_vals;
+      if (p.lat) { a.ssa = 1; a.lk_w_E = lk_w_E; a.lk_w_pbase = lk_w_pbase; a.w_cur_in = cursor.w; }
+      if (!published) publish(a);
+      a.pub_wwords = wwords;
+      if (int e = launch<PDL>("final", 1, k_final, lk_colv ? grid_for(lk_E, NT, s->sm_count) : 1, NT, 0, st, a)) return e;
     }
-    a.pub_wwords = wwords;
-    void* tkf = prof_begin(st);
-    launch_pdl(k_final, lk_colv ? grid_for(lk_E, NT, s->sm_count) : 1, NT, 0, st, a);
-    prof_end(tkf, "final", st, 1);
-    PYGB_LAUNCH_CHECK();
+    // table cleanup is stream-ordered after k_final; the host does not wait for it.  With
+    // PYGB200_S_DEFER_CLEANUP (homogeneous fast path) it rides along with pygb200_sampler_export_all instead.
+    s->cleanup_pending = (p.flags & PYGB200_S_DEFER_CLEANUP) && T == 1 && !p.direct && !p.v2;
+    s->last_direct = p.direct;
+    s->last_nodedup = p.nodedup;
+    s->nd_seeds = p.nodedup ? p.n_seeds[0] : 0;
+    if (p.v2) PYGB_CUDA(cudaEventRecord(s->final_ev, st));   // the table reset of this run waits for it on the side stream (below)
+    for (int t = 0; t < T && !s->cleanup_pending && !p.v2; ++t)
+      if (int e = cleanup_table(t, p.synced ? (i64)(s->types[t].slot.cap / 4) : p.node_cap[t], dst + list_word(t))) return e;
+    // pre-generation for the run after this one (decided when the previous run ended): launched now, on the side
+    // stream, while the GPU is busy with this run and the host has nothing to do but wait
+    if (s->mt_defer_target > 0) {
+      const int slot = s->mt_ev_next;
+      if (!s->mt_ev_pending[slot] && mt_request(s, s->mt_stream, s->mt_defer_target) == PYGB200_OK &&
+          cudaEventRecord(s->mt_ev[slot], s->mt_stream) == cudaSuccess) {
+        s->mt_ev_pending[slot] = true;
+        s->mt_ev_target[slot] = s->mt_defer_target;
+        s->mt_ev_next = slot ^ 1;
+      }
+      s->mt_defer_target = 0;
+    }
+    if (int e = wait_published()) return e;
+    if (pub_w_list >= 0) s->st_host[pub_w_list] = (i64)((u64)s->st_host[lay.words] & 0xffffffffffull);
+    const i64* hs = s->st_host;
+    PYGB_CHECK(hs[ST_ERROR] != 2, PYGB200_ERR_INTERNAL, "sampler: a peer rank did not reach a cross-GPU barrier in time (frontier-sharded run; PYGB200_XBARRIER_TIMEOUT_MS)");
+    if (int e = biased_error(hs[ST_ERROR])) return e;
+    PYGB_CHECK(hs[ST_ERROR] == 0, PYGB200_ERR_INTERNAL, "sampler: mt19937 stream buffer too small (internal bound violated)");
+    s->dirty = false;
+    read_counters(nodes_per_hop, edges_per_hop, n_nodes_out, n_edges_out);
+    if (p.v2) {
+      // reset the entries this run touched, on the side stream, behind k_final: the next run uses the other table and does
+      // not wait for it (the one after that does: clean_pending).  List lengths are host values by now.
+      PYGB_CUDA(cudaStreamWaitEvent(s->clean_stream, s->final_ev, 0));
+      for (int t = 0; t < T; ++t) {
+        auto& tb = s->types[t];
+        const i64 n = s->types[t].n_nodes;
+        if (n == 0) continue;
+        if (int e = launch<PLAIN>("cleanup", n, k_v2_cleanup, grid_for(n, NT, s->sm_count), NT, 0, s->clean_stream, tb.pk[s->v2_side].as<u64>(),
+                                  (const u32*)tb.vslot[s->v2_side].as<u32>(), n))
+          return e;
+      }
+      if (p.p2p && s->seedpk_bits[s->v2_side])
+        PYGB_CUDA(cudaMemsetAsync(s->seedpk[s->v2_side].p, 0xff, (size_t)8 << s->seedpk_bits[s->v2_side], s->clean_stream));
+      PYGB_CUDA(cudaEventRecord(s->clean_done[s->v2_side], s->clean_stream));
+      s->clean_pending[s->v2_side] = true;
+    }
+    memcpy(mt->state, hs + lay.o_mt, sizeof(mt->state));
+    mt->next = (int32_t)hs[ST_MT_NEXT];
+    mt->left = (int32_t)hs[ST_MT_LEFT];
+    // the stream persists: remember where it is and pre-generate what a run like this one will need,
+    // on the side stream (one CTA, overlaps the caller's work and the next run's first kernels)
+    s->st_o_list = list_word(0);
+    s->mt_expected = *mt;
+    s->mt_q = out0 + 256 * hs[ST_BLOCKS] + wwords;
+    s->mt_valid = true;
+    if (!p.synced && !p.weighted) {
+      const i64 target = std::min<i64>(s->raw_cap_words - 2 * MT_N, s->mt_q + 2 * run_outputs + 2 * MT_N);
+      // this run's kernels (which may extend the stream themselves) are done; the launch itself is left to the
+      // next run (see above) so that it costs no host time between two runs
+      s->mt_defer_target = target > s->mt_q ? target : 0;
+    }
+    return PYGB200_OK;
   }
-  // table cleanup is stream-ordered after k_final; the host does not wait for it.  With
-  // PYGB200_S_DEFER_CLEANUP (homogeneous fast path) it rides along with pygb200_sampler_export_all instead.
-  s->cleanup_pending = (flags & PYGB200_S_DEFER_CLEANUP) && T == 1 && !direct && !v2;
-  s->last_direct = direct;
-  s->last_nodedup = nodedup;
-  s->nd_seeds = nodedup ? n_seeds[0] : 0;
-  if (v2) PYGB_CUDA(cudaEventRecord(s->final_ev, st));   // the table reset of this run waits for it on the side stream (below)
-  for (int t = 0; t < T && !s->cleanup_pending && !v2; ++t) {
+  // the wide table of type t back to all-EMPTY: the *n_ptr listed nodes (<= n_grid) lose their entries
+  int cleanup_table(int t, i64 n_grid, const i64* n_ptr) {
     auto& tb = s->types[t];
-    const i64 cap_nodes = (i64)(tb.slot.cap / 4);
-    launch_pdl(k_cleanup, grid_for(synced ? cap_nodes : node_cap[t], NT, s->sm_count), NT, 0, st, tb.keys.as<u64>(), tb.vals.as<u64>(),
-               (const u32*)tb.slot.as<u32>(), (const i64*)(dst + (lat && cur_list[t].w >= 0 ? cur_list[t].w : lay.o_list + t)));
-    PYGB_LAUNCH_CHECK();
+    return launch<PDL>(nullptr, 0, k_cleanup, grid_for(n_grid, NT, s->sm_count), NT, 0, st, tb.keys.as<u64>(), tb.vals.as<u64>(),
+                       (const u32*)tb.slot.as<u32>(), n_ptr);
   }
-  // pre-generation for the run after this one (decided when the previous run ended): launched now, on the side
-  // stream, while the GPU is busy with this run and the host has nothing to do but wait
-  if (s->mt_defer_target > 0) {
-    const int slot = s->mt_ev_next;
-    if (!s->mt_ev_pending[slot] && mt_request(s, s->mt_stream, s->mt_defer_target) == PYGB200_OK &&
-        cudaEventRecord(s->mt_ev[slot], s->mt_stream) == cudaSuccess) {
-      s->mt_ev_pending[slot] = true;
-      s->mt_ev_target[slot] = s->mt_defer_target;
-      s->mt_ev_next = slot ^ 1;
-    }
-    s->mt_defer_target = 0;
-  }
-  {  // wait for k_final's flag (spin on mapped memory; keep an eye on the stream in case the run died)
+  // the state word that holds the node list length of type t at the end of the run
+  int list_word(int t) const { return p.lat && cur_list[t].w >= 0 ? cur_list[t].w : lay.o_list + t; }
+  // wait for k_final's flag (spin on mapped memory; keep an eye on the stream in case the run died)
+  int wait_published() {
     volatile i64* flag = s->st_host + lay.words;
     unsigned long long spins = 0;
     auto done = [&]() { return (((u64)*flag) >> 40) == ((u64)s->run_serial & 0xffffffull); };
@@ -2616,32 +2657,32 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
 #endif
     }
     std::atomic_thread_fence(std::memory_order_acquire);
+    return PYGB200_OK;
   }
-  if (pub_w_list >= 0) s->st_host[pub_w_list] = (i64)((u64)s->st_host[lay.words] & 0xffffffffffull);
-  const i64* hs = s->st_host;
-  PYGB_CHECK(hs[ST_ERROR] != 2, PYGB200_ERR_INTERNAL, "sampler: a peer rank did not reach a cross-GPU barrier in time (frontier-sharded run; PYGB200_XBARRIER_TIMEOUT_MS)");
-  if (int e = biased_error(hs[ST_ERROR])) return e;
-  PYGB_CHECK(hs[ST_ERROR] == 0, PYGB200_ERR_INTERNAL, "sampler: mt19937 stream buffer too small (internal bound violated)");
-  s->dirty = false;
-  if (lat) {   // counters from the write-once words of the schedule
-    auto val = [&](const Wd& x) { return x.w >= 0 ? hs[x.w] : x.c; };
-    for (int t = 0; t < T; ++t) {
-      const i64 n = val(cur_list[t]);
-      s->types[t].n_nodes = n;
-      if (n_nodes_out) n_nodes_out[t] = n;
-      if (nodes_per_hop) {
-        nodes_per_hop[(size_t)t * (L + 1)] = n_seeds[t];
-        for (int j = 1; j <= L; ++j)
-          nodes_per_hop[(size_t)t * (L + 1) + j] = val(list_end[(size_t)t * (L + 1) + j]) - val(list_end[(size_t)t * (L + 1) + j - 1]);
+  // node / edge counts of the run: from the write-once words of the latency schedule, else from the running counters
+  void read_counters(int64_t* nodes_per_hop, int64_t* edges_per_hop, int64_t* n_nodes_out, int64_t* n_edges_out) {
+    const int T = p.T, R = p.R, L = p.L;
+    const i64* hs = s->st_host;
+    if (p.lat) {
+      auto val = [&](const Wd& x) { return x.w >= 0 ? hs[x.w] : x.c; };
+      for (int t = 0; t < T; ++t) {
+        const i64 n = val(cur_list[t]);
+        s->types[t].n_nodes = n;
+        if (n_nodes_out) n_nodes_out[t] = n;
+        if (nodes_per_hop) {
+          nodes_per_hop[(size_t)t * (L + 1)] = p.n_seeds[t];
+          for (int j = 1; j <= L; ++j)
+            nodes_per_hop[(size_t)t * (L + 1) + j] = val(list_end[(size_t)t * (L + 1) + j]) - val(list_end[(size_t)t * (L + 1) + j - 1]);
+        }
       }
+      for (int r = 0; r < R; ++r) {
+        const i64 n = val(relcum[r]);
+        s->rels[r].n_edges = n;
+        if (n_edges_out) n_edges_out[r] = n;
+        if (edges_per_hop) for (int j = 0; j < L; ++j) edges_per_hop[(size_t)r * L + j] = eph_w[(size_t)r * L + j] >= 0 ? hs[eph_w[(size_t)r * L + j]] : 0;
+      }
+      return;
     }
-    for (int r = 0; r < R; ++r) {
-      const i64 n = val(relcum[r]);
-      s->rels[r].n_edges = n;
-      if (n_edges_out) n_edges_out[r] = n;
-      if (edges_per_hop) for (int j = 0; j < L; ++j) edges_per_hop[(size_t)r * L + j] = eph_w[(size_t)r * L + j] >= 0 ? hs[eph_w[(size_t)r * L + j]] : 0;
-    }
-  } else {
     for (int t = 0; t < T; ++t) {
       s->types[t].n_nodes = hs[lay.o_list + t];
       if (n_nodes_out) n_nodes_out[t] = hs[lay.o_list + t];
@@ -2653,40 +2694,40 @@ int sampler_run_impl(pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const 
       if (edges_per_hop) for (int j = 0; j < L; ++j) edges_per_hop[(size_t)r * L + j] = hs[lay.o_eph + r * L + j];
     }
   }
-  if (v2) {
-    // reset the entries this run touched, on the side stream, behind k_final: the next run uses the other table and does
-    // not wait for it (the one after that does: clean_pending).  List lengths are host values by now.
-    PYGB_CUDA(cudaStreamWaitEvent(s->clean_stream, s->final_ev, 0));
-    for (int t = 0; t < T; ++t) {
-      auto& tb = s->types[t];
-      const i64 n = s->types[t].n_nodes;
-      if (n == 0) continue;
-      void* tkc = prof_begin(s->clean_stream);
-      k_v2_cleanup<<<grid_for(n, NT, s->sm_count), NT, 0, s->clean_stream>>>(tb.pk[s->v2_side].as<u64>(), (const u32*)tb.vslot[s->v2_side].as<u32>(), n);
-      prof_end(tkc, "cleanup", s->clean_stream, n);
-      PYGB_LAUNCH_CHECK();
-    }
-    if (p2p && s->seedpk_bits[s->v2_side])
-      PYGB_CUDA(cudaMemsetAsync(s->seedpk[s->v2_side].p, 0xff, (size_t)8 << s->seedpk_bits[s->v2_side], s->clean_stream));
-    PYGB_CUDA(cudaEventRecord(s->clean_done[s->v2_side], s->clean_stream));
-    s->clean_pending[s->v2_side] = true;
+
+  int run(pygb200_mt19937* mt, int64_t* nodes_per_hop, int64_t* edges_per_hop, int64_t* n_nodes_out, int64_t* n_edges_out) {
+    if (int e = workspace()) return e;
+    if (int e = mt_stream(mt)) return e;
+    if (int e = init_state()) return e;
+    if (int e = seeds()) return e;
+    s->run_serial += 1;
+    if (int e = p.lat ? hops_latency() : p.synced ? hops_synced() : hops_bounded()) return e;
+    return finish(mt, nodes_per_hop, edges_per_hop, n_nodes_out, n_edges_out);
   }
-  memcpy(mt->state, hs + lay.o_mt, sizeof(mt->state));
-  mt->next = (int32_t)hs[ST_MT_NEXT];
-  mt->left = (int32_t)hs[ST_MT_LEFT];
-  // the stream persists: remember where it is and pre-generate what a run like this one will need,
-  // on the side stream (one CTA, overlaps the caller's work and the next run's first kernels)
-  s->st_o_list = lat && cur_list[0].w >= 0 ? cur_list[0].w : lay.o_list;
-  s->mt_expected = *mt;
-  s->mt_q = out0 + 256 * hs[ST_BLOCKS] + wwords;
-  s->mt_valid = true;
-  if (!synced && !weighted) {
-    const i64 target = std::min<i64>(s->raw_cap_words - 2 * MT_N, s->mt_q + 2 * run_outputs + 2 * MT_N);
-    // this run's kernels (which may extend the stream themselves) are done; the launch itself is left to the
-    // next run (see above) so that it costs no host time between two runs
-    s->mt_defer_target = target > s->mt_q ? target : 0;
-  }
-  return PYGB200_OK;
+};
+
+// The checks every run entry point makes (`fn` names it in their messages), then the run, under the sampler's mutex.
+int sampler_run_impl(const char* fn, pygb200_sampler* s, int32_t T, int32_t R, int32_t L, const pygb200_relation* rels,
+                     const void* const* seeds, const int64_t* n_seeds, const int64_t* num_neighbors, unsigned flags,
+                     pygb200_mt19937* mt, int64_t* nodes_per_hop, int64_t* edges_per_hop, int64_t* n_nodes_out,
+                     int64_t* n_edges_out, void* stream, const pygb200_shard* shard, const pygb200_temporal* temporal,
+                     const void* const* edge_weight, int32_t weight_dtype) {
+  PYGB_CHECK(s && seeds && n_seeds && mt && (rels || R == 0) && (num_neighbors || L == 0 || R == 0), PYGB200_ERR_ARG,
+             std::string(fn) + ": null argument");
+  PYGB_CHECK(T >= 1 && T <= 1024 && R >= 0 && L >= 0, PYGB200_ERR_ARG, std::string(fn) + ": bad T/R/L");
+  PYGB_CHECK(weight_dtype == PYGB200_F32, PYGB200_ERR_UNSUPPORTED,
+             "biased sampling: float32 edge weights only (the reference's random stream and key arithmetic depend on the weight dtype)");
+  std::lock_guard<std::mutex> lock(s->mu);
+  // the output binding is one-shot: it is consumed here, before any check can return early, so that a failed run
+  // never leaves pointers to arrays its caller is about to free (ADVICE r1)
+  const bool bound_armed = s->bound.armed;
+  s->bound.armed = false;
+  s->last_direct = false;
+  RunPlan p;
+  if (int e = make_plan(p, s, bound_armed, T, R, L, rels, seeds, n_seeds, num_neighbors, flags, mt, shard, temporal, edge_weight)) return e;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (p.idx32) return Run<int32_t>{s, st, p}.run(mt, nodes_per_hop, edges_per_hop, n_nodes_out, n_edges_out);
+  return Run<int64_t>{s, st, p}.run(mt, nodes_per_hop, edges_per_hop, n_nodes_out, n_edges_out);
 }
 
 }  // namespace
@@ -2696,12 +2737,8 @@ extern "C" int pygb200_sampler_run(pygb200_sampler* s, int32_t T, int32_t R, int
                                    const int64_t* n_seeds, const int64_t* num_neighbors, unsigned flags,
                                    pygb200_mt19937* mt, int64_t* nodes_per_hop, int64_t* edges_per_hop,
                                    int64_t* n_nodes_out, int64_t* n_edges_out, void* stream) {
-  PYGB_CHECK(s && seeds && n_seeds && mt && (rels || R == 0) && (num_neighbors || L == 0 || R == 0), PYGB200_ERR_ARG,
-             "pygb200_sampler_run: null argument");
-  PYGB_CHECK(T >= 1 && T <= 1024 && R >= 0 && L >= 0, PYGB200_ERR_ARG, "pygb200_sampler_run: bad T/R/L");
-  std::lock_guard<std::mutex> lock(s->mu);
-  return sampler_run_impl(s, T, R, L, rels, seeds, n_seeds, num_neighbors, flags, mt, nodes_per_hop, edges_per_hop,
-                          n_nodes_out, n_edges_out, (cudaStream_t)stream, nullptr, nullptr);
+  return sampler_run_impl("pygb200_sampler_run", s, T, R, L, rels, seeds, n_seeds, num_neighbors, flags, mt, nodes_per_hop,
+                          edges_per_hop, n_nodes_out, n_edges_out, stream, nullptr, nullptr, nullptr, PYGB200_F32);
 }
 
 extern "C" int pygb200_sampler_run_temporal(pygb200_sampler* s, int32_t T, int32_t R, int32_t L,
@@ -2710,12 +2747,8 @@ extern "C" int pygb200_sampler_run_temporal(pygb200_sampler* s, int32_t T, int32
                                             pygb200_mt19937* mt, int64_t* nodes_per_hop, int64_t* edges_per_hop,
                                             int64_t* n_nodes_out, int64_t* n_edges_out, void* stream,
                                             const pygb200_temporal* temporal) {
-  PYGB_CHECK(s && seeds && n_seeds && mt && (rels || R == 0) && (num_neighbors || L == 0 || R == 0), PYGB200_ERR_ARG,
-             "pygb200_sampler_run_temporal: null argument");
-  PYGB_CHECK(T >= 1 && T <= 1024 && R >= 0 && L >= 0, PYGB200_ERR_ARG, "pygb200_sampler_run_temporal: bad T/R/L");
-  std::lock_guard<std::mutex> lock(s->mu);
-  return sampler_run_impl(s, T, R, L, rels, seeds, n_seeds, num_neighbors, flags, mt, nodes_per_hop, edges_per_hop,
-                          n_nodes_out, n_edges_out, (cudaStream_t)stream, nullptr, temporal);
+  return sampler_run_impl("pygb200_sampler_run_temporal", s, T, R, L, rels, seeds, n_seeds, num_neighbors, flags, mt, nodes_per_hop,
+                          edges_per_hop, n_nodes_out, n_edges_out, stream, nullptr, temporal, nullptr, PYGB200_F32);
 }
 
 extern "C" int pygb200_sampler_run_weighted(pygb200_sampler* s, int32_t T, int32_t R, int32_t L,
@@ -2724,14 +2757,8 @@ extern "C" int pygb200_sampler_run_weighted(pygb200_sampler* s, int32_t T, int32
                                             pygb200_mt19937* mt, int64_t* nodes_per_hop, int64_t* edges_per_hop,
                                             int64_t* n_nodes_out, int64_t* n_edges_out, void* stream,
                                             const void* const* edge_weight, int32_t weight_dtype) {
-  PYGB_CHECK(s && seeds && n_seeds && mt && (rels || R == 0) && (num_neighbors || L == 0 || R == 0), PYGB200_ERR_ARG,
-             "pygb200_sampler_run_weighted: null argument");
-  PYGB_CHECK(T >= 1 && T <= 1024 && R >= 0 && L >= 0, PYGB200_ERR_ARG, "pygb200_sampler_run_weighted: bad T/R/L");
-  PYGB_CHECK(weight_dtype == PYGB200_F32, PYGB200_ERR_UNSUPPORTED,
-             "biased sampling: float32 edge weights only (the reference's random stream and key arithmetic depend on the weight dtype)");
-  std::lock_guard<std::mutex> lock(s->mu);
-  return sampler_run_impl(s, T, R, L, rels, seeds, n_seeds, num_neighbors, flags, mt, nodes_per_hop, edges_per_hop,
-                          n_nodes_out, n_edges_out, (cudaStream_t)stream, nullptr, nullptr, edge_weight);
+  return sampler_run_impl("pygb200_sampler_run_weighted", s, T, R, L, rels, seeds, n_seeds, num_neighbors, flags, mt, nodes_per_hop,
+                          edges_per_hop, n_nodes_out, n_edges_out, stream, nullptr, nullptr, edge_weight, weight_dtype);
 }
 
 extern "C" int pygb200_sampler_run_sharded(pygb200_sampler* s, int32_t T, int32_t R, int32_t L,
@@ -2740,12 +2767,8 @@ extern "C" int pygb200_sampler_run_sharded(pygb200_sampler* s, int32_t T, int32_
                                            pygb200_mt19937* mt, int64_t* nodes_per_hop, int64_t* edges_per_hop,
                                            int64_t* n_nodes_out, int64_t* n_edges_out, void* stream,
                                            const pygb200_shard* shard) {
-  PYGB_CHECK(s && seeds && n_seeds && mt && (rels || R == 0) && (num_neighbors || L == 0 || R == 0), PYGB200_ERR_ARG,
-             "pygb200_sampler_run_sharded: null argument");
-  PYGB_CHECK(T >= 1 && T <= 1024 && R >= 0 && L >= 0, PYGB200_ERR_ARG, "pygb200_sampler_run_sharded: bad T/R/L");
-  std::lock_guard<std::mutex> lock(s->mu);
-  return sampler_run_impl(s, T, R, L, rels, seeds, n_seeds, num_neighbors, flags, mt, nodes_per_hop, edges_per_hop,
-                          n_nodes_out, n_edges_out, (cudaStream_t)stream, shard, nullptr);
+  return sampler_run_impl("pygb200_sampler_run_sharded", s, T, R, L, rels, seeds, n_seeds, num_neighbors, flags, mt, nodes_per_hop,
+                          edges_per_hop, n_nodes_out, n_edges_out, stream, shard, nullptr, nullptr, PYGB200_F32);
 }
 
 extern "C" int pygb200_sampler_bounds(int32_t T, int32_t R, int32_t L, const pygb200_relation* rels,
@@ -2754,30 +2777,19 @@ extern "C" int pygb200_sampler_bounds(int32_t T, int32_t R, int32_t L, const pyg
   PYGB_CHECK(n_seeds && node_cap && (rels || R == 0) && (edge_cap || R == 0) && (num_neighbors || L == 0 || R == 0),
              PYGB200_ERR_ARG, "pygb200_sampler_bounds: null argument");
   PYGB_CHECK(T >= 1 && T <= 1024 && R >= 0 && L >= 0, PYGB200_ERR_ARG, "pygb200_sampler_bounds: bad T/R/L");
-  // same recurrence as the run's static bounds: frontier per (type, hop) -> edges per (relation, hop)
-  std::vector<i64> fb((size_t)T * (L + 1), 0);
-  for (int t = 0; t < T; ++t) fb[(size_t)t * (L + 1)] = n_seeds[t];
-  for (int r = 0; r < R; ++r) {
+  for (int r = 0; r < R; ++r)
     PYGB_CHECK(rels[r].src_type >= 0 && rels[r].src_type < T && rels[r].dst_type >= 0 && rels[r].dst_type < T,
                PYGB200_ERR_ARG, "pygb200_sampler_bounds: relation node type out of range");
-    edge_cap[r] = 0;
-  }
-  i64 total = 0;
   for (int h = 0; h < L; ++h)
-    for (int r = 0; r < R; ++r) {
-      const i64 k = num_neighbors[(size_t)r * L + h];
-      PYGB_CHECK(k >= 0, PYGB200_ERR_UNSUPPORTED, "pygb200_sampler_bounds: a fan-out of -1 has no static bound");
-      const i64 e = sat_mul(fb[(size_t)rels[r].src_type * (L + 1) + h], k);
-      edge_cap[r] = sat_add(edge_cap[r], e);
-      i64& nf = fb[(size_t)rels[r].dst_type * (L + 1) + h + 1];
-      nf = sat_add(nf, e);
-      total = sat_add(total, sat_mul(e, 4));
-    }
-  for (int t = 0; t < T; ++t) {
-    i64 c = 0;
-    for (int h = 0; h <= L; ++h) c = sat_add(c, fb[(size_t)t * (L + 1) + h]);
-    node_cap[t] = c;
-  }
+    for (int r = 0; r < R; ++r)
+      PYGB_CHECK(num_neighbors[(size_t)r * L + h] >= 0, PYGB200_ERR_UNSUPPORTED, "pygb200_sampler_bounds: a fan-out of -1 has no static bound");
+  // the run's static bounds, unclamped, with this function's own size limit (4 int64 words per edge)
+  std::vector<i64> fb, eb, nodes, edges;
+  static_bounds(T, R, L, rels, n_seeds, num_neighbors, fb, eb, nodes, edges);
+  i64 total = 0;
+  for (const i64 e : eb) total = sat_add(total, sat_mul(e, 4));
+  std::copy(nodes.begin(), nodes.end(), node_cap);
+  std::copy(edges.begin(), edges.end(), edge_cap);
   PYGB_CHECK(total <= ((i64)1 << 30), PYGB200_ERR_UNSUPPORTED, "pygb200_sampler_bounds: worst case too large for static sizing");
   return PYGB200_OK;
 }
@@ -2811,10 +2823,8 @@ extern "C" int pygb200_sampler_export_cumsum(pygb200_sampler* s, int64_t* out, v
   PYGB_CHECK(s->last_nodedup, PYGB200_ERR_ARG, "export_cumsum: the last run was not a PYGB200_S_NO_DEDUP run");
   cudaStream_t st = (cudaStream_t)stream;
   const i64 ne = s->rels[0].n_edges;
-  k_dist_cumsum<<<grid_for(s->nd_seeds + 1, NT, s->sm_count), NT, 0, st>>>(s->rec.as<NodeRec>(), s->tile_off.as<i64>(), s->nd_seeds, ne,
-                                                                            ne > 0 ? 1 : 0, reinterpret_cast<i64*>(out));
-  PYGB_LAUNCH_CHECK();
-  return PYGB200_OK;
+  return launch<PLAIN>(nullptr, 0, k_dist_cumsum, grid_for(s->nd_seeds + 1, NT, s->sm_count), NT, 0, st, s->rec.as<NodeRec>(),
+                       s->tile_off.as<i64>(), s->nd_seeds, ne, ne > 0 ? 1 : 0, reinterpret_cast<i64*>(out));
 }
 
 extern "C" int pygb200_sampler_export_edges(pygb200_sampler* s, int32_t rel, void* row_out, void* col_out,
@@ -2826,12 +2836,9 @@ extern "C" int pygb200_sampler_export_edges(pygb200_sampler* s, int32_t rel, voi
   if (n == 0) return PYGB200_OK;
   const int g = grid_for(n, NT, s->sm_count);
   const i64 *s0 = s->rels[rel].row.as<i64>(), *s1 = s->rels[rel].colv.as<i64>(), *s2 = s->rels[rel].eid.as<i64>();
-  void* tk = prof_begin(st);
-  if (index32) k_export3<int32_t><<<g, NT, 0, st>>>(s0, s1, s2, (int32_t*)row_out, (int32_t*)col_out, (int32_t*)edge_id_out, n);
-  else k_export3<int64_t><<<g, NT, 0, st>>>(s0, s1, s2, (int64_t*)row_out, (int64_t*)col_out, (int64_t*)edge_id_out, n);
-  prof_end(tk, "export", st, n);
-  PYGB_LAUNCH_CHECK();
-  return PYGB200_OK;
+  if (index32)
+    return launch<PLAIN>("export", n, k_export3<int32_t>, g, NT, 0, st, s0, s1, s2, (int32_t*)row_out, (int32_t*)col_out, (int32_t*)edge_id_out, n);
+  return launch<PLAIN>("export", n, k_export3<int64_t>, g, NT, 0, st, s0, s1, s2, (int64_t*)row_out, (int64_t*)col_out, (int64_t*)edge_id_out, n);
 }
 
 extern "C" int pygb200_sampler_export_all(pygb200_sampler* s, int32_t rel, void* row_out, void* col_out, void* edge_id_out,
@@ -2851,13 +2858,10 @@ extern "C" int pygb200_sampler_export_all(pygb200_sampler* s, int32_t rel, void*
   const i64* node = s->types[type].nodes.as<i64>();
   const i64* batch = s->disjoint ? s->types[type].batch.as<i64>() : nullptr;
   if (index32)
-    launch_pdl(k_export4<int32_t>, g, NT, 0, st, s0, s1, s2, (int32_t*)row_out, (int32_t*)col_out, (int32_t*)edge_id_out, ne, node,
-               batch, (int32_t*)node_id_out, nn, ck, cv, cs);
-  else
-    launch_pdl(k_export4<int64_t>, g, NT, 0, st, s0, s1, s2, (int64_t*)row_out, (int64_t*)col_out, (int64_t*)edge_id_out, ne, node,
-               batch, (int64_t*)node_id_out, nn, ck, cv, cs);
-  PYGB_LAUNCH_CHECK();
-  return PYGB200_OK;
+    return launch<PDL>(nullptr, 0, k_export4<int32_t>, g, NT, 0, st, s0, s1, s2, (int32_t*)row_out, (int32_t*)col_out, (int32_t*)edge_id_out,
+                       ne, node, batch, (int32_t*)node_id_out, nn, ck, cv, cs);
+  return launch<PDL>(nullptr, 0, k_export4<int64_t>, g, NT, 0, st, s0, s1, s2, (int64_t*)row_out, (int64_t*)col_out, (int64_t*)edge_id_out,
+                     ne, node, batch, (int64_t*)node_id_out, nn, ck, cv, cs);
 }
 
 extern "C" int pygb200_sampler_export_nodes(pygb200_sampler* s, int32_t type, void* node_id_out, int index32,
@@ -2871,15 +2875,11 @@ extern "C" int pygb200_sampler_export_nodes(pygb200_sampler* s, int32_t type, vo
   const i64* node = s->types[type].nodes.as<i64>();
   if (s->disjoint) {
     const i64* batch = s->types[type].batch.as<i64>();
-    if (index32) k_export_pairs<int32_t><<<g, NT, 0, st>>>(batch, node, (int32_t*)node_id_out, n);
-    else k_export_pairs<int64_t><<<g, NT, 0, st>>>(batch, node, (int64_t*)node_id_out, n);
-    PYGB_LAUNCH_CHECK();
-  } else if (index32) {
-    k_export<int32_t><<<g, NT, 0, st>>>(node, (int32_t*)node_id_out, n);
-    PYGB_LAUNCH_CHECK();
-  } else {
-    PYGB_CUDA(cudaMemcpyAsync(node_id_out, node, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
+    if (index32) return launch<PLAIN>(nullptr, 0, k_export_pairs<int32_t>, g, NT, 0, st, batch, node, (int32_t*)node_id_out, n);
+    return launch<PLAIN>(nullptr, 0, k_export_pairs<int64_t>, g, NT, 0, st, batch, node, (int64_t*)node_id_out, n);
   }
+  if (index32) return launch<PLAIN>(nullptr, 0, k_export<int32_t>, g, NT, 0, st, node, (int32_t*)node_id_out, n);
+  PYGB_CUDA(cudaMemcpyAsync(node_id_out, node, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
   return PYGB200_OK;
 }
 
